@@ -12,7 +12,7 @@ holds its own row shard (weak scaling): the job is ONE fit over N x rows per ste
 units of the 1-GPU workload (`value` = N fit-units / s; at N=1 plain fit()/s).  CCALoss is "replicas only"
 (per-replica batch statistics, as in the reference): N independent replicas.  Prints ONE JSON line on rank 0.
 
-CPU arms.  The reference is pure Python over LAPACK and /root/reference does not exist on the GPU box, so both CPU legs
+CPU arms.  The reference is pure Python over LAPACK and is not a dependency of this package, so both CPU legs
 run the oracle's line-by-line restatement of the reference algorithm (`kind: "port"`): `--impl reference` and the
 `cpu_baseline` object time the FULL workload (no row sampling, no extrapolation); a fit of configs[1] takes about a
 minute on the host cores, so the number of timed CPU fits is capped by a wall-clock budget (at least one, reported in
@@ -373,7 +373,7 @@ def run_ours(args):
         step_dev = lambda: est.fit(views)      # noqa: E731
         step_e2e = lambda: est.fit(host)       # noqa: E731
         h2d = sum(h.numel() * h.element_size() for h in host)
-        l2_note = f"inputs ({h2d / 1e6:.0f} MB per GPU) exceed the 126 MB L2; no explicit flush"
+        l2_note = f"inputs ({h2d / 1e6:.0f} MB per GPU) exceed the 50 MB L2 of the H100; no explicit flush"
     else:
         from cca_zoo_b200.deep import CCALoss
 
@@ -383,13 +383,17 @@ def run_ours(args):
         del raw
         zs = [h.to(dev).requires_grad_(True) for h in host]
         fn = CCALoss(eps=1e-5)
-        flush = torch.empty(160 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+        flush = torch.empty(160 << 20, dtype=torch.uint8, device=dev)   # > the 50 MB L2 of the H100
+
+        last_loss = [None]
 
         def step_dev():
             flush.zero_()                       # L2 flush between timed iterations (the batch itself is 2-16 MB)
             for z in zs:
                 z.grad = None
-            fn(zs).backward()
+            loss = fn(zs)
+            loss.backward()
+            last_loss[0] = loss.detach()
 
         grads_host = [torch.empty_like(h).pin_memory() for h in host]
         loss_host = torch.empty((), dtype=torch.float32).pin_memory()
@@ -406,7 +410,7 @@ def run_ours(args):
         h2d = sum(h.numel() * h.element_size() for h in host)
         l2_note = "a 160 MB buffer is overwritten between timed iterations (L2 flush); its 0.03 ms is inside the step"
 
-    # ---- device-resident arm (`value`) with live timing of the tcgen05 moment kernel ----
+    # ---- device-resident arm (`value`) with live timing of the tensor-core moment kernel ----
     for _ in range(args.warmup):
         step_dev()
     lib.ccab_profile_moments(1)
@@ -423,6 +427,15 @@ def run_ours(args):
     clocks = sampler.stop() if sampler else None
     lib.ccab_profile_moments(0)
     ms_per_step = total_ms / args.steps
+    if args.dump_outputs and rank == 0:
+        # what the timed path handed back in its last step, before the end-to-end leg refits
+        if est is not None:
+            dumped = {f"weights_{i}": w for i, w in enumerate(est.weights_)}
+            dumped.update({f"means_{i}": np.asarray(m) for i, m in enumerate(est.means_)})
+        else:
+            dumped = {"loss": last_loss[0].cpu().numpy().reshape(1)}
+            dumped.update({f"grad_{i}": z.grad.detach().cpu().numpy() for i, z in enumerate(zs)})
+        dump_outputs(args.dump_outputs, dumped)
     value = world / (ms_per_step * 1e-3)
 
     # ---- end-to-end arm: pinned host inputs -> public API -> result on the host ----
@@ -448,37 +461,30 @@ def run_ours(args):
     k1 = float(np.mean([m for m in k1_ms if m and m > 0])) if any(m and m > 0 for m in k1_ms) else None
     roof = None
     if model in ("rcca", "mcca"):
-        bf16 = peaks.get("bf16_tflops", 1590.0)
+        bf16 = peaks.get("bf16_tflops", 989.0)
         peak_src = "MEASURED_PEAKS.json bf16_tflops/2 (TF32 runs at half the dense bf16 rate)" if peaks else \
-            "fallback 1590/2 TFLOP/s (B200_PROFILING.md)"
+            "data sheet 989/2 TFLOP/s (H100 SXM dense BF16 / TF32 at 700 W; not a measured peak)"
         flops = n * D * (D + 1)  # algorithmic: symmetric product, SURVEY.md §8d (per rank)
-        passes = {"tf32x3": 3, "tf32x3b": 2}.get(args.precision, 1)
-        traffic = None
-        try:
-            with open(os.path.join(ROOT, "profiles", "k1_traffic.json")) as f:
-                tr = json.load(f)[f"{args.workload}:{args.precision}"]
-            traffic = tr["dram_bytes_read"] + tr["dram_bytes_write"]   # one ncu --set full capture, per launch
-        except Exception:
-            pass
+        passes = {"tf32x3": 3, "tf32x3b": 3}.get(args.precision, 1)
         if k1:
             ach = flops / (k1 * 1e-3) / 1e12
-            kname = {"tf32x3b": "moments_x3b_persist_kernel (persistent CTA pairs; 2 bf16 cross-term + 2 tf32 MMAs per 16 samples)",
-                     "tf32x3": "moments_tf32_2cta_kernel<X3> (3 tf32 MMAs per k-step)"}.get(
-                         args.precision, "moments_tf32_2cta_kernel")
+            kname = {"tf32x3b": "moments_wgmma_kernel<X3> (3 tf32 wgmmas per k-step)",
+                     "tf32x3": "moments_wgmma_kernel<X3> (3 tf32 wgmmas per k-step)"}.get(
+                         args.precision, "moments_wgmma_kernel")
             roof = {"bound": "tensor", "kernel": kname, "achieved": ach, "peak": bf16 / 2,
-                    "unit": "TFLOP/s", "frac": ach / (bf16 / 2), "traffic": traffic, "kernel_ms": k1,
+                    "unit": "TFLOP/s", "frac": ach / (bf16 / 2), "traffic": None, "kernel_ms": k1,
                     "mma_passes": passes, "algorithmic_flops": flops, "algorithmic_bytes": n * D * 4,
                     "frac_of_issued": passes * ach / (bf16 / 2), "peak_source": peak_src,
                     "share_of_step": k1 / ms_per_step}
     else:
         # config 3 is HBM / latency bound (SURVEY.md §8d): algorithmic bytes = z read by the moment pass, z read again
         # and the gradients written by the backward = 3 x (2 x batch x width x 4)
-        hbm = peaks.get("hbm_gbs", 6575.0)
+        hbm = peaks.get("hbm_gbs", 3350.0)
         abytes = 3 * 2 * n * W["dims"][0] * 4
         ach = abytes / (ms_per_step * 1e-3) / 1e9
         roof = {"bound": "hbm", "kernel": "whole step (moments, small solves, backward products)", "achieved": ach,
                 "peak": hbm, "unit": "GB/s", "frac": ach / hbm, "traffic": None, "algorithmic_bytes": abytes,
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback (B200_PROFILING.md)",
+                "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "data sheet 3.35 TB/s (H100 SXM HBM3)",
                 "note": "latency bound: the step is a chain of small dependent launches; frac is reported, not chased"}
 
     line = {
@@ -512,6 +518,20 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(dirname: str, arrays: dict, limit_bytes: int = 64 << 20):
+    """Write each array as DIR/<name>.npy in float32 or float64.  Arrays are small for every workload here (weights,
+    means, a loss and its gradients); the limit guards the total."""
+    os.makedirs(dirname, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        total += a.nbytes
+        if total > limit_bytes:
+            raise RuntimeError(f"--dump-outputs: more than {limit_bytes >> 20} MB of outputs")
+        np.save(os.path.join(dirname, f"{name}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -522,6 +542,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline / parity legs")
     ap.add_argument("--no-e2e", action="store_true", help="profiling only: skip the end-to-end leg (the line is then "
                                                           "not a valid bench line)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy")
     ap.add_argument("--workload", default="rcca", choices=sorted(WORKLOADS),
                     help="rcca = BASELINE configs[1] (the headline); mcca4 = configs[3] shard; ccaloss64 / "
                          "ccaloss512 = configs[2] at the two readings of its width")

@@ -1,7 +1,7 @@
-"""cca_zoo_b200 -- B200-native drop-in for the covariance -> eigensolve hot path of cca_zoo.
+"""cca_zoo_b200 -- H100-native drop-in for the covariance -> eigensolve hot path of cca_zoo.
 
 ``cca_zoo_b200.linear`` mirrors ``cca_zoo.linear`` (CCA, rCCA, PLS, MCCA, GCCA, PartialCCA, GRCCA) and
 ``cca_zoo_b200.deep.objectives`` mirrors ``cca_zoo.deep.objectives`` (CCALoss, MCCALoss, GCCALoss).
-All arithmetic runs in hand-written sm_100a kernels (libccab200.so, include/ccab200.h).
+All arithmetic runs in hand-written sm_90a kernels (libccab200.so, include/ccab200.h).
 """
 __version__ = "0.1.0"

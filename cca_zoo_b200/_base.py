@@ -1,4 +1,4 @@
-"""Base class of the B200 estimators: the reference's sklearn surface (cca_zoo/_base.py:19-258) with
+"""Base class of the H100 estimators: the reference's sklearn surface (cca_zoo/_base.py:19-258) with
 the fit-time arithmetic moved to the GPU.
 
 Drop-in contract kept from the reference:
@@ -115,7 +115,7 @@ class BaseModel(BaseEstimator, ABC):
     def _device(self) -> torch.device:
         if not torch.cuda.is_available():
             raise RuntimeError(
-                "cca_zoo_b200 needs a CUDA device (sm_100a); there is no CPU fallback.  "
+                "cca_zoo_b200 needs a CUDA device (sm_90a); there is no CPU fallback.  "
                 "Use the reference cca_zoo package on CPU-only machines."
             )
         if self.device is None:
@@ -338,7 +338,7 @@ class BaseModel(BaseEstimator, ABC):
         """Project views with the fitted weights: ``(v - mean_) @ weights_`` per view (cca_zoo/_base.py:108-123).
 
         CUDA tensors, and host inputs above ``_device_score_threshold`` elements, are projected on the device:
-        ``Z_i = X_i W_i - 1 (mean_i^T W_i)`` is one GEMM per view (tcgen05 for float32, DMMA for float64) whose output
+        ``Z_i = X_i W_i - 1 (mean_i^T W_i)`` is one GEMM per view (wgmma for float32, DMMA for float64) whose output
         is pre-loaded with the mean term, so neither a centred copy of the data nor a second pass exists.  Returns
         numpy arrays like the reference."""
         check_is_fitted(self)

@@ -55,8 +55,8 @@ static int require_device() {
   if (e != cudaSuccess) return cuda_fail(e, "cudaGetDevice (no CUDA device: libccab200 has no CPU fallback)");
   int major = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) {
-    set_error("libccab200 is built for sm_100a only; device %d has compute capability major %d", dev, major);
+  if (major != 9) {
+    set_error("libccab200 is built for sm_90a (Hopper) only; device %d has compute capability major %d", dev, major);
     return -10;
   }
   return 0;
@@ -92,7 +92,7 @@ int ccab_moments(int dtype, int precision, int n_views, const void* const* views
   CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
   CCAB_CHECK_ARG(precision >= 0 && precision <= 3, "bad precision %d", precision);
   CCAB_CHECK_ARG(!(dtype == CCAB_F64 && precision != CCAB_PREC_EXACT),
-                 "float64 inputs support CCAB_PREC_EXACT only (tcgen05 has no f64 kind)");
+                 "float64 inputs support CCAB_PREC_EXACT only (the TF32 tensor-core path has no f64 kind)");
   CCAB_CHECK_ARG(views && dims && lds && moments && workspace, "null pointer argument");
   ColumnLayout L;
   int rc = make_layout(n_views, dims, &L);
@@ -350,7 +350,7 @@ int ccab_gemm(int dtype, int transa, int transb, int m, int n, int k, double alp
   int rc = require_device();
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (dtype == CCAB_F32) {   // tensor pipe (tcgen05, 3xTF32) when TMA can address the operands, FMA tiles otherwise
+  if (dtype == CCAB_F32) {   // tensor pipe (wgmma, 3xTF32) when TMA can address the operands, FMA tiles otherwise
     GemmArgs<float> g;
     g.transa = transa; g.transb = transb; g.m = m; g.n = n; g.k = k; g.alpha = (float)alpha; g.beta = (float)beta;
     g.A = static_cast<const float*>(A); g.lda = lda; g.B = static_cast<const float*>(B); g.ldb = ldb;
@@ -669,16 +669,8 @@ double ccab_profile_moments_last_ms(void) { return (double)moments_profile_last_
 int ccab_debug_set(const char* key, int value) {
   if (!key) return -1;
   TcDebug& d = tc_debug();
-  if (!strcmp(key, "lbo_bytes")) d.lbo_bytes = value;
-  else if (!strcmp(key, "sbo_bytes")) d.sbo_bytes = value;
-  else if (!strcmp(key, "tma_dtype")) d.tma_dtype = value;
-  else if (!strcmp(key, "force_splits")) d.force_splits = value;
-  else if (!strcmp(key, "tc_variant")) d.variant = value < 0 ? 0 : value;
-  else if (!strcmp(key, "tc_kc")) d.kc = value < 0 ? 0 : value;
-  else if (!strcmp(key, "tc_dry_run")) d.dry_run = value < 0 ? 0 : value;
-  else if (!strcmp(key, "x3_split")) d.x3_split = value < 0 ? 0 : value;
+  if (!strcmp(key, "force_splits")) d.force_splits = value;
   else if (!strcmp(key, "f64_simt")) d.f64_simt = value < 0 ? 0 : value;
-  else if (!strcmp(key, "x3b_oneshot")) d.x3b_oneshot = value < 0 ? 0 : value;
   else if (!strcmp(key, "gemm_force_fma")) xgemm_force_fma() = value < 0 ? 0 : value;
   else if (!strcmp(key, "gemm_split")) xgemm_split_enabled() = value < 0 ? 1 : value;
   else if (!strcmp(key, "jacobi_inner_sweeps")) jacobi_inner_sweeps() = value;

@@ -1,6 +1,6 @@
-// Shared device/host helpers for libccab200 (sm_100a only).
+// Shared device/host helpers for libccab200 (sm_90a, Hopper).
 //
-// PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor) and tcgen05 (alloc / mma / commit / ld).
+// PTX wrappers for the warpgroup MMA (wgmma) and the shared-memory staging of its operands.
 // Everything is hand-written inline PTX; no CUTLASS/CuTe dependency.
 #pragma once
 
@@ -46,278 +46,122 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
 
 // ---------------------------------------------------------------------------------------------
-// mbarrier
+// Hopper warpgroup MMA (wgmma, sm_90a): four warps issue one asynchronous MMA whose operands are read from shared
+// memory through the async proxy and whose fp32 accumulators live in the registers of the warpgroup.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void fence_mbar_init() {
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P1;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, P1;\n\t"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Bounded wait: a protocol bug must trap (-> CUDA error on the host), never hang the GPU box.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 22)) {  // each failed try_wait already sleeps ~ a microsecond
-      printf("ccab: mbarrier wait timed out (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y,
-             threadIdx.x);
-      __trap();
-    }
-  }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving reads of the accumulators above the wait that retires the MMAs writing them
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---------------------------------------------------------------------------------------------
-// TMA
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tma_prefetch_desc(const void* map) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* map, uint64_t* bar, int c0,
-                                            int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
+// Shared-memory matrix descriptor of a K-major tile with 128-byte swizzle: one 128-byte row (32 fp32 reduction
+// indices) per M / N index, 8-row groups 1024 B apart (SBO); LBO is unused by swizzled K-major layouts.  The tile
+// base must be 1024-byte aligned; a k-step of 8 tf32 values advances the start address by 32 bytes.
+__device__ __forceinline__ uint64_t wgmma_desc_k128(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)1 << 62);
 }
 
-// ---------------------------------------------------------------------------------------------
-// tcgen05
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// whole warp, .sync.aligned
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// single thread
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// d (64 x N fp32 fragment of the warpgroup) += A (64 x 8, K-major) * B (N x 8, K-major)^T in TF32.
+// Fragment element r of a thread: row 16*(warp % 4) + lane/4 + 8*((r/2) % 2), column 8*(r/4) + 2*(lane % 4) + r % 2.
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t desc_a, uint64_t desc_b);
 
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread t <-> lane base+t)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t* r) {
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float* d, uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-        "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t tmem_ld_32x32b_x1(uint32_t taddr) {
-  uint32_t r;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-  return r;
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(1));
 }
 
-// ---------------------------------------------------------------------------------------------
-// CTA-pair (cta_group::2) variants: two CTAs of a cluster (same TPC) execute one M=256 MMA; each holds
-// its own 128 rows of A and half of the N columns of B in its own shared memory.
-// ---------------------------------------------------------------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address -> CTA 0
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster (release at cluster scope)
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+template <>
+__device__ __forceinline__ void wgmma_tf32<128>(float* d, uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-// executed by both CTAs; the transaction bytes are credited to the LEADER CTA's mbarrier
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const void* map, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-// one warp in EACH CTA of the pair, same smem offset
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// single thread of the leader CTA
-__device__ __forceinline__ void umma_tf32_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// kind::f16 (bf16 / fp16 operands, fp32 accumulate) on the CTA pair: K = 16 per instruction, twice the TF32 rate
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives (once the previously issued MMAs retire) on the mbarrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(1));
 }
 
-// 64-bit shared-memory matrix descriptor (sm_100 "version 1").
-//   start address  bits [ 0,14)  (addr  >> 4)
-//   leading  byte offset bits [16,30) (bytes >> 4)
-//   stride   byte offset bits [32,46) (bytes >> 4)
-//   version        bits [46,48) = 1
-//   layout type    bits [61,64) : 0 none, 2 = SWIZZLE_128B, 4 = 64B, 6 = 32B
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(layout_type & 7) << 61;
-  return d;
-}
-
-// 32-bit instruction descriptor for kind::tf32, fp32 accumulate, both operands MN-major ("transposed":
-// the reduction index is the strided one in shared memory).
-__host__ __device__ constexpr uint32_t umma_idesc_tf32_mn(uint32_t M, uint32_t N) {
-  return (1u << 4)      // c_format  = F32
-         | (2u << 7)    // a_format  = TF32
-         | (2u << 10)   // b_format  = TF32
-         | (1u << 15)   // a_major   = MN
-         | (1u << 16)   // b_major   = MN
-         | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-
-// 3xTF32 residual: the tensor core TRUNCATES fp32 operands to TF32 (measured, tools/probe_trunc.py), so a raw fp32
-// array is its own "hi" operand; lo = rna_tf32(x - trunc(x)) carries the next 11 bits (x = hi + lo + O(2^-21 |x|)).
+// 3xTF32 split: hi = x with the low 13 mantissa bits cleared (what the tensor core reads of an fp32 operand),
+// lo = rna_tf32(x - hi) carries the next 11 bits (x = hi + lo + O(2^-21 |x|)).
+__device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float(__float_as_uint(v) & 0xFFFFE000u); }
 __device__ __forceinline__ float tf32_residual(float v) {
-  const float hi = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
   uint32_t l;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(v - hi));
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(v - tf32_hi(v)));
   return __uint_as_float(l);
 }
 
-// general instruction descriptor for kind::tf32 (fp32 accumulate): *_kmajor = the reduction index is the
-// contiguous one of that operand's shared-memory tile
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(uint32_t M, uint32_t N, bool a_kmajor, bool b_kmajor) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((a_kmajor ? 0u : 1u) << 15) | ((b_kmajor ? 0u : 1u) << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
+// Byte offset of the 16-byte chunk holding reduction indices 4*kg .. 4*kg+3 of row `row` in a K-major tile with
+// 128-byte swizzle (see wgmma_desc_k128).
+__device__ __forceinline__ uint32_t k128_offset(int row, int kg) {
+  return (uint32_t)row * 128u + ((uint32_t)(kg ^ (row & 7)) << 4);
 }
 
-// 4-D TMA tile load (inner, outer, batch, batch2)
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const void* map, uint64_t* bar, int c0, int c1, int c2,
-                                            int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
+// Stages a ROWS x 32 slice of an operand (ROWS output rows or columns, 32 reduction indices) from global memory into
+// a K-major swizzled shared tile, as hi and (X3) lo copies.  Each of the 256 threads of the block owns ROWS / 32 items
+// of one row and four consecutive reduction indices.  KMAJ: the reduction index is contiguous in memory (element
+// (r, k) at X[r * ld + k], item lanes walk k); otherwise it is the strided one (element (r, k) at X[k * ld + r],
+// item lanes walk r).  Out-of-range elements (r >= rows, k >= ks) are zero.  Loading and storing are separate
+// steps so that the global loads of the next slice are in flight while the tensor cores work on this one.
+template <bool KMAJ, int ROWS>
+struct TileStager {
+  static constexpr int kItems = ROWS * 8 / 256;
+  float v[kItems][4];
 
-// instruction descriptor for kind::f16 with BF16 operands, fp32 accumulate, both operands MN-major
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_mn(uint32_t M, uint32_t N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
+  __device__ __forceinline__ static int item_row(int i) { return KMAJ ? i >> 3 : i % ROWS; }
+  __device__ __forceinline__ static int item_kg(int i) { return KMAJ ? i & 7 : i / ROWS; }
 
-// 3-D TMA tile load (inner, outer, batch)
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* map, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
+  // X points at element (0, 0) of the slice; rows / ks: valid extent; vec: KMAJ rows may be read as float4
+  __device__ __forceinline__ void load(const float* X, int64_t ld, int rows, int ks, bool vec) {
+#pragma unroll
+    for (int j = 0; j < kItems; ++j) {
+      const int i = threadIdx.x + 256 * j;
+      const int r = item_row(i), k = 4 * item_kg(i);
+      if (KMAJ) {
+        const float* src = X + (int64_t)r * ld + k;
+        if (vec && r < rows && k + 4 <= ks) {
+          const float4 q = __ldg(reinterpret_cast<const float4*>(src));
+          v[j][0] = q.x; v[j][1] = q.y; v[j][2] = q.z; v[j][3] = q.w;
+        } else {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) v[j][e] = (r < rows && k + e < ks) ? __ldg(src + e) : 0.f;
+        }
+      } else {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[j][e] = (r < rows && k + e < ks) ? __ldg(X + (int64_t)(k + e) * ld + r) : 0.f;
+      }
+    }
+  }
+
+  template <bool X3>
+  __device__ __forceinline__ void store(uint8_t* hi, uint8_t* lo) const {
+#pragma unroll
+    for (int j = 0; j < kItems; ++j) {
+      const int i = threadIdx.x + 256 * j;
+      const uint32_t off = k128_offset(item_row(i), item_kg(i));
+      *reinterpret_cast<float4*>(hi + off) =
+          make_float4(tf32_hi(v[j][0]), tf32_hi(v[j][1]), tf32_hi(v[j][2]), tf32_hi(v[j][3]));
+      if (X3)
+        *reinterpret_cast<float4*>(lo + off) = make_float4(tf32_residual(v[j][0]), tf32_residual(v[j][1]),
+                                                           tf32_residual(v[j][2]), tf32_residual(v[j][3]));
+    }
+  }
+};
 
 #endif  // __CUDACC__
 

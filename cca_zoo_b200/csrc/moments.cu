@@ -1,11 +1,9 @@
 // K1: block moments M = X^T X (+ column sums) of the hstacked views, upper block triangle only.
 //
-//   * moments_tf32_kernel : tcgen05.mma kind::tf32, both operands MN-major straight out of row-major X
-//     (TMA boxes of 32 columns x KC rows, 128B rows swizzled in 32B chunks), fp32 accumulators in TMEM, warp-specialised
-//     (TMA producer / single-thread MMA issuer / 4 epilogue warps), split over the sample axis.
-//     Optional 3xTF32 (raw operand = hi by hardware truncation, materialised residual lo, 3 MMAs per k-step)
-//     for fp32-grade accuracy.
-//     Column sums ride on the same pipeline as one extra N=16 MMA against a block of ones.
+//   * moments_wgmma_kernel : Hopper wgmma (TF32, fp32 accumulators in registers), 128 x 128 tiles of the upper
+//     block triangle, split over the sample axis.  The sample slices are transposed into K-major swizzled shared
+//     tiles by the staging stores.  Optional 3xTF32 (hi / lo copies staged in shared memory, 3 MMAs per k-step) for
+//     fp32-grade accuracy.  Column sums are exact fp32 sums of the staged values.
 //   * moments_simt_kernel : exact FMA (fp32) tile kernel, the non-tensor reference path;
 //     moments_dmma_kernel : float64 inputs on the fp64 tensor pipe (mma.sync m8n8k4.f64).
 //   * reduce / covariance kernels (K2): fixed-order sum of the split partials into a double
@@ -46,7 +44,7 @@ int make_layout(int n_views, const int64_t* dims, ColumnLayout* L) {
   return 0;
 }
 
-// optional timing of the tcgen05 kernel alone (bench.py roofline): events on the launching stream
+// optional timing of the tensor-core moment kernel alone (bench.py roofline): events on the launching stream
 static bool g_prof_on = false;
 static cudaEvent_t g_prof_e0 = nullptr, g_prof_e1 = nullptr;
 static bool g_prof_valid = false;
@@ -67,972 +65,135 @@ float moments_profile_last_ms() {
 }
 
 TcDebug& tc_debug() {
-  static TcDebug d = {-1, -1, -1, 0, 0, 0, 0, 0, 0, 0};
+  static TcDebug d = {0, 0};
   return d;
 }
 
 // =============================================================================================
-// tcgen05 kernel
+// wgmma kernel
 // =============================================================================================
-struct alignas(64) TcParams {
-  CUtensorMap maps[2 * kMaxViews];  // [v] raw / hi operand, [8+v] lo operand (3xTF32)
-  float* partial;                   // [S][Dp][Dp]
-  float* partial_sum;               // [S][Dp]
-  int total_chunks, chunks_per_split, num_splits;
-  int nblocks, Dp;
-  int lbo_bytes, sbo_bytes;
-  int row_tile_start[kMaxBlocks + 1];
-  int blk_col0[kMaxBlocks];
+// One CTA = one 128 x 128 tile (A block bi, B block bj >= bi) of M over one split of the sample axis.  Its 256 threads
+// stage each 32-sample slice of both column blocks into K-major swizzled shared tiles (the sample index is the
+// strided one of row-major X, so the transpose is done by the staging stores), double-buffered: the global loads of
+// slice c + 1 are in flight while the two warpgroups run the wgmmas of slice c, each on 64 rows of the tile.
+// The 3xTF32 mode stages hi and lo copies and issues lo*hi + hi*lo + hi*hi per k-step.  Column sums are exact fp32
+// sums of the staged values, taken by the diagonal tiles.
+struct WgParams {
+  const float* view_ptr[kMaxViews];
+  int64_t view_ld[kMaxViews];
+  int view_dim[kMaxViews];
   uint8_t blk_view[kMaxBlocks];
+  int blk_col0[kMaxBlocks];
+  float* partial;      // [S][Dp][Dp]
+  float* partial_sum;  // [S][Dp]
+  int64_t n_rows, rows_per_split;
+  int nblocks, Dp;
 };
-static_assert(sizeof(TcParams) <= 4096, "kernel parameter space");
+static_assert(sizeof(WgParams) <= 4096, "kernel parameter space");
 
-constexpr int kTcThreads = 192;  // warp0 TMA, warp1 MMA, warps2-5 epilogue
-constexpr int kTcStages = 4;
-constexpr int kSumCol = 256;     // TMEM column of the column-sum accumulator (N = 16)
-// MN-major TF32 operands admit exactly one shared-memory layout: 128-byte rows swizzled in 32-byte
-// chunks (descriptor layout type 1 = SWIZZLE_128B_BASE32B, TMA CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B).
-// Canonical form (16-byte units): ((8,n),(4,k)) : ((1,LBO),(8,SBO)) -- a 32-float row per reduction
-// index, 4-row groups SBO apart, 32-column atoms LBO apart.  Verified on hardware by tools/umma_unit.cu.
-constexpr uint32_t kUmmaLayout = 1;
+constexpr int kWgThreads = 256;
+constexpr int kWgKC = 32;                  // samples per slice = one 128-byte K-major row
+constexpr int kWgTile = kBlk * kWgKC * 4;  // bytes of one staged 128 x 32 operand copy
 
-template <int KC, bool X3>
-struct TcCfg {
-  static constexpr int kAtom = KC * 128;               // one 32-col x KC-row box
-  static constexpr int kSet = 12 * kAtom;              // A (4 atoms) + B (8 atoms)
-  static constexpr int kStage = (X3 ? 2 : 1) * kSet;
-  static constexpr int kSmem = kTcStages * kStage + 1024 /*ones*/ + 1024 /*align slack*/ + 128;
+template <bool X3>
+struct WgCfg {
+  static constexpr int kOps = X3 ? 2 : 1;           // hi (+ lo) copy of each operand
+  static constexpr int kStage = 2 * kOps * kWgTile;  // A copies, then B copies
+  static constexpr int kSmem = 2 * kStage + 1024;    // two stages + alignment slack
 };
 
-template <int KC, bool X3>
-__global__ void __launch_bounds__(kTcThreads, 1)
-moments_tf32_kernel(const __grid_constant__ TcParams p) {
-  using Cfg = TcCfg<KC, X3>;
+template <bool X3>
+__global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __grid_constant__ WgParams p) {
+  using Cfg = WgCfg<X3>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* ones = smem + kTcStages * Cfg::kStage;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(ones + 1024);
-  uint64_t* empty_bar = full_bar + kTcStages;
-  uint64_t* tmem_full_bar = empty_bar + kTcStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
+  __shared__ float colsum_hi[kBlk];
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  // ---- tile decode: blockIdx.x -> (A block, up to two B blocks) ----
-  const int tile = blockIdx.x;
-  int bi = 0;
-  while (p.row_tile_start[bi + 1] <= tile) ++bi;
-  const int t_in_row = tile - p.row_tile_start[bi];
-  const int bj0 = bi + 2 * t_in_row;
-  const int nB = (bj0 + 1 < p.nblocks) ? 2 : 1;
-  const int N = nB * 128;
-  const bool do_sum = (t_in_row == 0);
+  int t = blockIdx.x, bi = 0, rowlen = p.nblocks;   // tile decode over the upper block triangle
+  while (t >= rowlen) { t -= rowlen; ++bi; --rowlen; }
+  const int bj = bi + t;
+  const bool diag = bi == bj;
   const int split = blockIdx.y;
-  const int c0 = split * p.chunks_per_split;
-  const int c1 = min(c0 + p.chunks_per_split, p.total_chunks);
-  const bool has_work = c1 > c0;
+  const int64_t r0 = (int64_t)split * p.rows_per_split;
+  const int64_t r1 = min(r0 + p.rows_per_split, p.n_rows);
+  const int nch = r1 > r0 ? (int)((r1 - r0 + kWgKC - 1) / kWgKC) : 0;
 
-  // ---- one-time setup ----
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kTcStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    mbar_init(tmem_full_bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0 && lane == 0) {
-    for (int v = 0; v < kMaxViews; ++v) {
-      // harmless for unused slots: they hold a copy of view 0's map
-      tma_prefetch_desc(&p.maps[v]);
-      if (X3) tma_prefetch_desc(&p.maps[kMaxViews + v]);
-    }
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  if (warp >= 2) {
-    float* o = reinterpret_cast<float*>(ones);
-    for (int i = threadIdx.x - 64; i < 256; i += 128) o[i] = 1.0f;
-    fence_proxy_async_smem();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  const int vA = p.blk_view[bi], vB = p.blk_view[bj];
+  const float* XA = p.view_ptr[vA] + p.blk_col0[bi];
+  const float* XB = p.view_ptr[vB] + p.blk_col0[bj];
+  const int64_t ldA = p.view_ld[vA], ldB = p.view_ld[vB];
+  const int colsA = p.view_dim[vA] - p.blk_col0[bi], colsB = p.view_dim[vB] - p.blk_col0[bj];
 
-  if (warp == 0) {
-    // ================= TMA producer =================
-    if (has_work && elect_one()) {
-      const int vA = p.blk_view[bi], colA = p.blk_col0[bi];
-      int vB[2], colB[2];
-      for (int b = 0; b < 2; ++b) {
-        int bj = min(bj0 + b, p.nblocks - 1);
-        vB[b] = p.blk_view[bj];
-        colB[b] = p.blk_col0[bj];
-      }
-      const uint32_t bytes = (X3 ? 2u : 1u) * (4u + 4u * nB) * Cfg::kAtom;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int c = c0; c < c1; ++c) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        mbar_arrive_expect_tx(&full_bar[stage], bytes);
-        uint8_t* st = smem + stage * Cfg::kStage;
-        const int row = c * KC;
+  TileStager<false, kBlk> sa, sb;
+  float csum = 0.f;   // column threadIdx.x % 128 of a diagonal tile, this thread's reduction indices
+  auto load = [&](int c) {
+    const int64_t r = r0 + (int64_t)c * kWgKC;
+    const int ks = (int)(r1 - r < kWgKC ? r1 - r : kWgKC);
+    sa.load(XA + r * ldA, ldA, colsA, ks, false);
+    if (!diag) sb.load(XB + r * ldB, ldB, colsB, ks, false);
+  };
+  auto store = [&](int buf) {
+    uint8_t* st = smem + buf * Cfg::kStage;
+    sa.template store<X3>(st, st + kWgTile);
+    if (!diag) sb.template store<X3>(st + Cfg::kOps * kWgTile, st + (Cfg::kOps + 1) * kWgTile);
+    if (diag) {
 #pragma unroll
-        for (int o = 0; o < (X3 ? 2 : 1); ++o) {
-          uint8_t* base = st + o * Cfg::kSet;
-          const CUtensorMap* mA = &p.maps[o * kMaxViews + vA];
-#pragma unroll
-          for (int a = 0; a < 4; ++a) tma_load_2d(base + a * Cfg::kAtom, mA, &full_bar[stage], colA + 32 * a, row);
-          for (int b = 0; b < nB; ++b) {
-            const CUtensorMap* mB = &p.maps[o * kMaxViews + vB[b]];
-#pragma unroll
-            for (int a = 0; a < 4; ++a)
-              tma_load_2d(base + (4 + 4 * b + a) * Cfg::kAtom, mB, &full_bar[stage], colB[b] + 32 * a, row);
-          }
-        }
-        if (++stage == kTcStages) { stage = 0; phase ^= 1; }
-      }
+      for (int j = 0; j < TileStager<false, kBlk>::kItems; ++j) csum += (sa.v[j][0] + sa.v[j][1]) + (sa.v[j][2] + sa.v[j][3]);
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer (one elected thread) =================
-    if (has_work) {
-      const uint32_t idesc_main = umma_idesc_tf32_mn(128, N);
-      const uint32_t idesc_sum = umma_idesc_tf32_mn(128, 16);
-      const uint32_t lbo = p.lbo_bytes, sbo = p.sbo_bytes;
-      const uint64_t ones_desc = umma_smem_desc(smem_u32(ones), lbo, sbo, kUmmaLayout);
-      const uint64_t descA0 = umma_smem_desc(smem_u32(smem), lbo, sbo, kUmmaLayout);
-      const uint64_t descB0 = umma_smem_desc(smem_u32(smem) + 4 * Cfg::kAtom, lbo, sbo, kUmmaLayout);
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t acc = 0u;
-      for (int c = c0; c < c1; ++c) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t so = (uint64_t)((stage * Cfg::kStage) >> 4);
-#pragma unroll
-          for (int kk = 0; kk < KC / 8; ++kk) {
-            const uint64_t a_hi = descA0 + so + (uint64_t)(kk * 64);
-            const uint64_t b_hi = descB0 + so + (uint64_t)(kk * 64);
-            if (X3) {
-              const uint64_t a_lo = a_hi + (uint64_t)(Cfg::kSet >> 4);
-              const uint64_t b_lo = b_hi + (uint64_t)(Cfg::kSet >> 4);
-              // small cross terms first, then the leading term
-              umma_tf32(tmem_base, a_lo, b_hi, idesc_main, acc);
-              umma_tf32(tmem_base, a_hi, b_lo, idesc_main, 1u);
-              umma_tf32(tmem_base, a_hi, b_hi, idesc_main, 1u);
-              if (do_sum) {
-                umma_tf32(tmem_base + kSumCol, a_lo, ones_desc, idesc_sum, acc);
-                umma_tf32(tmem_base + kSumCol, a_hi, ones_desc, idesc_sum, 1u);
-              }
-            } else {
-              umma_tf32(tmem_base, a_hi, b_hi, idesc_main, acc);
-              if (do_sum) umma_tf32(tmem_base + kSumCol, a_hi, ones_desc, idesc_sum, acc);
-            }
-            acc = 1u;
-          }
-          umma_commit(&empty_bar[stage]);  // frees the smem stage once these MMAs retire
-        }
-        acc = 1u;
-        __syncwarp();
-        if (++stage == kTcStages) { stage = 0; phase ^= 1; }
-      }
-      if (elect_one()) umma_commit(tmem_full_bar);
-      __syncwarp();
-    }
-  } else {
-    // ================= epilogue: TMEM -> registers -> global partials =================
-    const int g = warp & 3;           // TMEM lane group this warp may touch
-    const int m = g * 32 + lane;      // accumulator row = column of the A block
-    float* prow = p.partial + ((size_t)split * p.Dp + (size_t)bi * 128 + m) * p.Dp;
-    if (has_work) {
-      mbar_wait(tmem_full_bar, 0);
-      tc_fence_after();
-    }
-    for (int cc = 0; cc < N / 32; ++cc) {
-      uint32_t r[32];
-      if (has_work) {
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(g * 32) << 16) + cc * 32, r);
-        tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) r[i] = 0u;
-      }
-      const int bj = bj0 + (cc >> 2);
-      float4* dst = reinterpret_cast<float4*>(prow + (size_t)bj * 128 + (cc & 3) * 32);
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        dst[q] = make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]),
-                             __uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3]));
-    }
-    if (do_sum) {
-      uint32_t sv = 0u;
-      if (has_work) {
-        sv = tmem_ld_32x32b_x1(tmem_base + ((uint32_t)(g * 32) << 16) + kSumCol);
-        tmem_ld_wait();
-      }
-      p.partial_sum[(size_t)split * p.Dp + bi * 128 + m] = __uint_as_float(sv);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// =============================================================================================
-// CTA-pair variant: tcgen05.mma.cta_group::2, 256 x 256 output tiles (pair-blocks of two 128-column
-// blocks).  CTA r of the cluster loads A block 2I+r and B block 2J+r (32 KB per stage instead of 48 KB),
-// the leader's single MMA thread drives both tensor cores, every B half is read from shared memory once for
-// both SMs: shared-memory and L2->SM traffic per MAC drop by 1.5x against the 1-CTA 128x256 tile.
-// =============================================================================================
-struct alignas(64) TcParams2 {
-  CUtensorMap maps[2 * kMaxViews];
-  float* partial;      // [S][Dp2][Dp2]
-  float* partial_sum;  // [S][Dp2]
-  int total_chunks, chunks_per_split, num_splits;
-  int nblocks, nb2, Dp2;
-  int lbo_bytes, sbo_bytes;
-  int dry_run;  // debug: after the first ring fill, recycle stale stages without TMA (isolates the MMA rate)
-  int blk_col0[kMaxBlocks + 2];      // entry nblocks (and nblocks+1) = dummy block: out-of-bounds -> zeros
-  uint8_t blk_view[kMaxBlocks + 2];
-};
-static_assert(sizeof(TcParams2) <= 4096, "kernel parameter space");
-
-template <int KC, bool X3, int NS>
-struct Tc2Cfg {
-  static constexpr int kStages = NS;
-  static constexpr int kAtom = KC * 128;
-  static constexpr int kSet = 8 * kAtom;  // A (4 atoms) + B half (4 atoms)
-  static constexpr int kStage = (X3 ? 2 : 1) * kSet;
-  static constexpr int kSmem = NS * kStage + 1024 + 1024 + 256;
-};
-
-template <int KC, bool X3, int NS>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kTcThreads, 1)
-moments_tf32_2cta_kernel(const __grid_constant__ TcParams2 p) {
-  using Cfg = Tc2Cfg<KC, X3, NS>;
-  constexpr int kTc2Stages = NS;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* ones = smem + kTc2Stages * Cfg::kStage;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(ones + 1024);
-  uint64_t* empty_bar = full_bar + kTc2Stages;
-  uint64_t* tmem_full_bar = empty_bar + kTc2Stages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  int t = blockIdx.x >> 1, I = 0, rowlen = p.nb2;
-  while (t >= rowlen) { t -= rowlen; ++I; --rowlen; }
-  const int J = I + t;
-  const bool do_sum = (I == J);
-  const int blkA = min(2 * I + (int)rank, p.nblocks);  // index nblocks = dummy (zeros)
-  const int blkB = min(2 * J + (int)rank, p.nblocks);
-  const int split = blockIdx.y;
-  const int c0 = split * p.chunks_per_split;
-  const int c1 = min(c0 + p.chunks_per_split, p.total_chunks);
-  const bool has_work = c1 > c0;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kTc2Stages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    mbar_init(tmem_full_bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0 && lane == 0) {
-    for (int v = 0; v < kMaxViews; ++v) {
-      tma_prefetch_desc(&p.maps[v]);
-      if (X3) tma_prefetch_desc(&p.maps[kMaxViews + v]);
-    }
-  }
-  if (warp == 1) tmem_alloc_2sm(tmem_slot, 512);
-  if (warp >= 2) {
-    float* o = reinterpret_cast<float*>(ones);
-    for (int i = threadIdx.x - 64; i < 256; i += 128) o[i] = 1.0f;
-    fence_proxy_async_smem();
-  }
-  tc_fence_before();
-  cluster_sync_all();  // both CTAs' barriers are initialised before any cross-CTA arrive / TMA credit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ================= TMA producer (both CTAs, each loads its own halves) =================
-    if (has_work && elect_one()) {
-      const int vA = p.blk_view[blkA], colA = p.blk_col0[blkA];
-      const int vB = p.blk_view[blkB], colB = p.blk_col0[blkB];
-      const uint32_t bytes_pair = 2u * (X3 ? 2u : 1u) * 8u * Cfg::kAtom;  // both CTAs credit the leader's barrier
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int c = c0; c < c1; ++c) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        if (p.dry_run && c - c0 >= kTc2Stages) {
-          if (leader) mbar_arrive(&full_bar[stage]);
-          if (++stage == kTc2Stages) { stage = 0; phase ^= 1; }
-          continue;
-        }
-        if (leader) mbar_arrive_expect_tx(&full_bar[stage], bytes_pair);
-        uint8_t* st = smem + stage * Cfg::kStage;
-        const int row = c * KC;
-#pragma unroll
-        for (int o = 0; o < (X3 ? 2 : 1); ++o) {
-          uint8_t* base = st + o * Cfg::kSet;
-          const CUtensorMap* mA = &p.maps[o * kMaxViews + vA];
-          const CUtensorMap* mB = &p.maps[o * kMaxViews + vB];
-#pragma unroll
-          for (int a = 0; a < 4; ++a) tma_load_2d_2sm(base + a * Cfg::kAtom, mA, &full_bar[stage], colA + 32 * a, row);
-#pragma unroll
-          for (int a = 0; a < 4; ++a)
-            tma_load_2d_2sm(base + (4 + a) * Cfg::kAtom, mB, &full_bar[stage], colB + 32 * a, row);
-        }
-        if (++stage == kTc2Stages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer: one thread of the LEADER CTA drives both SMs =================
-    if (leader && has_work) {
-      const uint32_t idesc_main = umma_idesc_tf32_mn(256, 256);
-      const uint32_t idesc_sum = umma_idesc_tf32_mn(256, 16);
-      const uint32_t lbo = p.lbo_bytes, sbo = p.sbo_bytes;
-      const uint64_t ones_desc = umma_smem_desc(smem_u32(ones), lbo, sbo, kUmmaLayout);
-      // descriptor of stage 0 / k-step 0; later ones differ only in the 14-bit start-address field
-      const uint64_t descA0 = umma_smem_desc(smem_u32(smem), lbo, sbo, kUmmaLayout);
-      const uint64_t descB0 = umma_smem_desc(smem_u32(smem) + 4 * Cfg::kAtom, lbo, sbo, kUmmaLayout);
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t acc = 0u;
-      for (int c = c0; c < c1; ++c) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t so = (uint64_t)((stage * Cfg::kStage) >> 4);
-#pragma unroll
-          for (int kk = 0; kk < KC / 8; ++kk) {
-            const uint64_t a_hi = descA0 + so + (uint64_t)(kk * 64);
-            const uint64_t b_hi = descB0 + so + (uint64_t)(kk * 64);
-            if (X3) {
-              const uint64_t a_lo = a_hi + (uint64_t)(Cfg::kSet >> 4);
-              const uint64_t b_lo = b_hi + (uint64_t)(Cfg::kSet >> 4);
-              umma_tf32_2sm(tmem_base, a_lo, b_hi, idesc_main, acc);
-              umma_tf32_2sm(tmem_base, a_hi, b_lo, idesc_main, 1u);
-              umma_tf32_2sm(tmem_base, a_hi, b_hi, idesc_main, 1u);
-              if (do_sum) {
-                umma_tf32_2sm(tmem_base + kSumCol, a_lo, ones_desc, idesc_sum, acc);
-                umma_tf32_2sm(tmem_base + kSumCol, a_hi, ones_desc, idesc_sum, 1u);
-              }
-            } else {
-              umma_tf32_2sm(tmem_base, a_hi, b_hi, idesc_main, acc);
-              if (do_sum) umma_tf32_2sm(tmem_base + kSumCol, a_hi, ones_desc, idesc_sum, acc);
-            }
-            acc = 1u;
-          }
-          umma_commit_2sm(&empty_bar[stage], 3);  // frees this stage in BOTH CTAs
-        }
-        acc = 1u;
-        __syncwarp();
-        if (++stage == kTc2Stages) { stage = 0; phase ^= 1; }
-      }
-      if (elect_one()) umma_commit_2sm(tmem_full_bar, 3);
-      __syncwarp();
-    }
-  } else {
-    // ================= epilogue (both CTAs): own 128 accumulator rows x 256 columns =================
-    const int g = warp & 3;
-    const int m = g * 32 + lane;
-    const size_t prow_idx = (size_t)(2 * I + rank) * 128 + m;
-    float* prow = p.partial + ((size_t)split * p.Dp2 + prow_idx) * p.Dp2;
-    if (has_work) {
-      mbar_wait(tmem_full_bar, 0);
-      tc_fence_after();
-    }
-    for (int cc = 0; cc < 8; ++cc) {
-      uint32_t r[32];
-      if (has_work) {
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(g * 32) << 16) + cc * 32, r);
-        tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) r[i] = 0u;
-      }
-      float4* dst = reinterpret_cast<float4*>(prow + (size_t)(2 * J + (cc >> 2)) * 128 + (cc & 3) * 32);
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        dst[q] = make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]),
-                             __uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3]));
-    }
-    if (do_sum) {
-      uint32_t sv = 0u;
-      if (has_work) {
-        sv = tmem_ld_32x32b_x1(tmem_base + ((uint32_t)(g * 32) << 16) + kSumCol);
-        tmem_ld_wait();
-      }
-      p.partial_sum[(size_t)split * p.Dp2 + prow_idx] = __uint_as_float(sv);
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();  // nobody frees TMEM / exits while the pair is still using either CTA's resources
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, 512);
-  }
-}
-
-// =============================================================================================
-// 3xTF32 with the two CROSS TERMS on the bf16 pipe ("tf32x3b"): x = hi + lo with hi = trunc_tf32(x); the leading term
-// hi*hi runs as kind::tf32 from the raw array (the hardware truncates), the cross terms lo*hi + hi*lo as kind::f16
-// MMAs on bf16 copies bhi = bf16(hi), blo = bf16(lo) (K = 16 per instruction at twice the TF32 rate: 2 instead of 3
-// units of tensor work per sample, and half the shared-memory bytes for the cross operands).  Error of one accumulator
-// run: 3e-7 relative (3xTF32: 1.3e-7, single pass: 7.5e-4; tools/next/emulate_x3_bf16_cross.py) -- still fp32 grade.
-// bf16 MN-major operands: 64-column TMA boxes (SWIZZLE_128B), descriptor layout SWIZZLE_128B, LBO = KC*128 between
-// 64-column atoms, SBO = 1024 between 8-row groups, 2048 B per K = 16 step (probed on hardware:
-// tools/next/umma_bf16_mn_probe.cu, profiles/r2_bf16_mn_probe.txt).
-// =============================================================================================
-struct alignas(64) TcParams3 {
-  CUtensorMap maps[3 * kMaxViews];   // [v] raw fp32, [8+v] bhi (bf16), [16+v] blo (bf16)
-  float* partial;
-  float* partial_sum;
-  int total_chunks, chunks_per_split, num_splits;
-  int nblocks, nb2, Dp2;
-  int ntiles, total_units;           // persistent kernel: units = (tile, split) pairs, dealt round-robin to the CTA pairs
-  int blk_col0[kMaxBlocks + 2];
-  uint8_t blk_view[kMaxBlocks + 2];
-};
-static_assert(sizeof(TcParams3) <= 4096, "kernel parameter space");
-
-template <int NS>
-struct Tc3Cfg {
-  static constexpr int KC = 16;
-  static constexpr int kAtom = KC * 128;        // 32 fp32 columns x 16 rows  ==  64 bf16 columns x 16 rows
-  static constexpr int kRaw = 8 * kAtom;        // A (4 atoms) + B half (4 atoms), fp32
-  static constexpr int kBf = 2 * kAtom;         // one bf16 operand of 128 columns
-  static constexpr int kStage = kRaw + 4 * kBf; // + A.bhi, A.blo, B.bhi, B.blo
-  static constexpr int kSmem = NS * kStage + 3072 + 1024 + 256;
-};
-
-template <int NS>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kTcThreads, 1)
-moments_x3b_2cta_kernel(const __grid_constant__ TcParams3 p) {
-  using Cfg = Tc3Cfg<NS>;
-  constexpr int KC = Cfg::KC;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* ones = smem + NS * Cfg::kStage;          // 1024 B of 1.0f, then 2048 B of bf16 1.0 (two 8-row groups)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(ones + 3072);
-  uint64_t* empty_bar = full_bar + NS;
-  uint64_t* tmem_full_bar = empty_bar + NS;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  int t = blockIdx.x >> 1, I = 0, rowlen = p.nb2;
-  while (t >= rowlen) { t -= rowlen; ++I; --rowlen; }
-  const int J = I + t;
-  const bool do_sum = (I == J);
-  const int blkA = min(2 * I + (int)rank, p.nblocks);
-  const int blkB = min(2 * J + (int)rank, p.nblocks);
-  const int split = blockIdx.y;
-  const int c0 = split * p.chunks_per_split;
-  const int c1 = min(c0 + p.chunks_per_split, p.total_chunks);
-  const bool has_work = c1 > c0;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < NS; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    mbar_init(tmem_full_bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0 && lane == 0) {
-    for (int v = 0; v < 3 * kMaxViews; ++v) tma_prefetch_desc(&p.maps[v]);
-  }
-  if (warp == 1) tmem_alloc_2sm(tmem_slot, 512);
-  if (warp >= 2) {
-    float* o = reinterpret_cast<float*>(ones);
-    uint32_t* ob = reinterpret_cast<uint32_t*>(ones + 1024);
-    for (int i = threadIdx.x - 64; i < 512; i += 128) {
-      if (i < 256) o[i] = 1.0f;
-      ob[i] = 0x3F803F80u;   // two bf16 ones
-    }
-    fence_proxy_async_smem();
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ================= TMA producer (both CTAs, each loads its own halves) =================
-    if (has_work && elect_one()) {
-      const int vA = p.blk_view[blkA], colA = p.blk_col0[blkA];
-      const int vB = p.blk_view[blkB], colB = p.blk_col0[blkB];
-      const uint32_t bytes_pair = 2u * Cfg::kStage;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int c = c0; c < c1; ++c) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        if (leader) mbar_arrive_expect_tx(&full_bar[stage], bytes_pair);
-        uint8_t* st = smem + stage * Cfg::kStage;
-        const int row = c * KC;
-#pragma unroll
-        for (int a = 0; a < 4; ++a) tma_load_2d_2sm(st + a * Cfg::kAtom, &p.maps[vA], &full_bar[stage], colA + 32 * a, row);
-#pragma unroll
-        for (int a = 0; a < 4; ++a)
-          tma_load_2d_2sm(st + (4 + a) * Cfg::kAtom, &p.maps[vB], &full_bar[stage], colB + 32 * a, row);
-        uint8_t* bf = st + Cfg::kRaw;
-#pragma unroll
-        for (int o = 0; o < 2; ++o) {      // 0: bhi, 1: blo
-#pragma unroll
-          for (int a = 0; a < 2; ++a) {
-            tma_load_2d_2sm(bf + (o * 2 + a) * Cfg::kAtom, &p.maps[(1 + o) * kMaxViews + vA], &full_bar[stage],
-                            colA + 64 * a, row);
-            tma_load_2d_2sm(bf + (4 + o * 2 + a) * Cfg::kAtom, &p.maps[(1 + o) * kMaxViews + vB], &full_bar[stage],
-                            colB + 64 * a, row);
-          }
-        }
-        if (++stage == NS) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer: one thread of the LEADER CTA drives both SMs =================
-    if (leader && has_work) {
-      const uint32_t idesc_tf = umma_idesc_tf32_mn(256, 256), idesc_tf_sum = umma_idesc_tf32_mn(256, 16);
-      const uint32_t idesc_bf = umma_idesc_bf16_mn(256, 256), idesc_bf_sum = umma_idesc_bf16_mn(256, 16);
-      const uint32_t sb = smem_u32(smem);
-      const uint64_t ones_tf = umma_smem_desc(smem_u32(ones), KC * 128, 512, kUmmaLayout);
-      const uint64_t ones_bf = umma_smem_desc(smem_u32(ones) + 1024, KC * 128, 1024, 2);
-      const uint64_t dA_tf = umma_smem_desc(sb, KC * 128, 512, kUmmaLayout);
-      const uint64_t dB_tf = umma_smem_desc(sb + 4 * Cfg::kAtom, KC * 128, 512, kUmmaLayout);
-      const uint64_t dA_bhi = umma_smem_desc(sb + Cfg::kRaw, KC * 128, 1024, 2);
-      const uint64_t dA_blo = umma_smem_desc(sb + Cfg::kRaw + Cfg::kBf, KC * 128, 1024, 2);
-      const uint64_t dB_bhi = umma_smem_desc(sb + Cfg::kRaw + 2 * Cfg::kBf, KC * 128, 1024, 2);
-      const uint64_t dB_blo = umma_smem_desc(sb + Cfg::kRaw + 3 * Cfg::kBf, KC * 128, 1024, 2);
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t acc = 0u;
-      for (int c = c0; c < c1; ++c) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t so = (uint64_t)((stage * Cfg::kStage) >> 4);
-          // small cross terms first (one K = 16 bf16 MMA each), then the leading term (two K = 8 tf32 MMAs)
-          umma_f16_2sm(tmem_base, dA_blo + so, dB_bhi + so, idesc_bf, acc);
-          umma_f16_2sm(tmem_base, dA_bhi + so, dB_blo + so, idesc_bf, 1u);
-          umma_tf32_2sm(tmem_base, dA_tf + so, dB_tf + so, idesc_tf, 1u);
-          umma_tf32_2sm(tmem_base, dA_tf + so + 64, dB_tf + so + 64, idesc_tf, 1u);
-          if (do_sum) {
-            umma_f16_2sm(tmem_base + kSumCol, dA_blo + so, ones_bf, idesc_bf_sum, acc);
-            umma_tf32_2sm(tmem_base + kSumCol, dA_tf + so, ones_tf, idesc_tf_sum, 1u);
-            umma_tf32_2sm(tmem_base + kSumCol, dA_tf + so + 64, ones_tf, idesc_tf_sum, 1u);
-          }
-          umma_commit_2sm(&empty_bar[stage], 3);
-        }
-        acc = 1u;
-        __syncwarp();
-        if (++stage == NS) { stage = 0; phase ^= 1; }
-      }
-      if (elect_one()) umma_commit_2sm(tmem_full_bar, 3);
-      __syncwarp();
-    }
-  } else {
-    // ================= epilogue (both CTAs): own 128 accumulator rows x 256 columns =================
-    const int g = warp & 3;
-    const int m = g * 32 + lane;
-    const size_t prow_idx = (size_t)(2 * I + rank) * 128 + m;
-    float* prow = p.partial + ((size_t)split * p.Dp2 + prow_idx) * p.Dp2;
-    if (has_work) {
-      mbar_wait(tmem_full_bar, 0);
-      tc_fence_after();
-    }
-    for (int cc = 0; cc < 8; ++cc) {
-      uint32_t r[32];
-      if (has_work) {
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(g * 32) << 16) + cc * 32, r);
-        tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) r[i] = 0u;
-      }
-      float4* dst = reinterpret_cast<float4*>(prow + (size_t)(2 * J + (cc >> 2)) * 128 + (cc & 3) * 32);
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        dst[q] = make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]),
-                             __uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3]));
-    }
-    if (do_sum) {
-      uint32_t sv = 0u;
-      if (has_work) {
-        sv = tmem_ld_32x32b_x1(tmem_base + ((uint32_t)(g * 32) << 16) + kSumCol);
-        tmem_ld_wait();
-      }
-      p.partial_sum[(size_t)split * p.Dp2 + prow_idx] = __uint_as_float(sv);
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, 512);
-  }
-}
-
-// pre-pass of the tf32x3b mode: bhi = bf16(trunc_tf32(x)), blo = bf16(x - trunc_tf32(x)); reads n*d*4 B, writes n*d*4 B
-__device__ __forceinline__ uint32_t bf16_rn_bits(float v) {
-  uint32_t u = __float_as_uint(v);
-  u += 0x7FFFu + ((u >> 16) & 1u);
-  return u >> 16;
-}
-__global__ void tf32_bf16_split_kernel(const float* __restrict__ x, int64_t n, int d, int64_t ldx,
-                                       uint16_t* __restrict__ bhi, uint16_t* __restrict__ blo, int64_t ldo, int vec4) {
-  if (vec4) {
-    const int d4 = d >> 2;
-    const int64_t total = n * (int64_t)d4;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-      const int64_t r = i / d4;
-      const int c = (int)(i - r * d4) << 2;
-      const float4 v = *reinterpret_cast<const float4*>(x + r * ldx + c);
-      const float vv[4] = {v.x, v.y, v.z, v.w};
-      uint32_t h[4], l[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float hi = __uint_as_float(__float_as_uint(vv[q]) & 0xFFFFE000u);
-        h[q] = bf16_rn_bits(hi);
-        l[q] = bf16_rn_bits(vv[q] - hi);
-      }
-      *reinterpret_cast<uint2*>(bhi + r * ldo + c) = make_uint2(h[0] | (h[1] << 16), h[2] | (h[3] << 16));
-      *reinterpret_cast<uint2*>(blo + r * ldo + c) = make_uint2(l[0] | (l[1] << 16), l[2] | (l[3] << 16));
-    }
-  } else {
-    const int64_t total = n * (int64_t)d;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-      const int64_t r = i / d;
-      const int c = (int)(i - r * d);
-      const float v = x[r * ldx + c];
-      const float hi = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
-      bhi[r * ldo + c] = (uint16_t)bf16_rn_bits(hi);
-      blo[r * ldo + c] = (uint16_t)bf16_rn_bits(v - hi);
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Persistent form of the kernel above (default): one CTA pair per SM pair walks the (tile, split) units
-// u = pair, pair + npairs, ... with ONE continuous TMA / MMA pipeline and TWO 256-column accumulators in TMEM, so the
-// epilogue of unit i (TMEM -> registers -> split partial in HBM) runs under the MMAs of unit i + 1 and the per-unit
-// start-up (barrier init, TMEM allocation, cluster sync, ring fill) is paid once.  Consecutive units of a pair share
-// their sample rows with the units the other pairs are processing (tile index fastest), which keeps the operand
-// re-reads in L2.  The two accumulators leave no room for the 16-column sum accumulator: the column sums come from
-// the pre-pass (tf32_bf16_split_sums_kernel), exactly in fp32.
-//   tmem_full_bar[b]  (each CTA)  : MMA commit, multicast       -> epilogue warps of both CTAs
-//   tmem_empty_bar[b] (leader CTA): 4 epilogue warps x 2 CTAs   -> MMA thread (remote arrive from the peer)
-// ---------------------------------------------------------------------------------------------
-template <int NS>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kTcThreads, 1)
-moments_x3b_persist_kernel(const __grid_constant__ TcParams3 p) {
-  using Cfg = Tc3Cfg<NS>;
-  constexpr int KC = Cfg::KC;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + NS * Cfg::kStage);
-  uint64_t* empty_bar = full_bar + NS;
-  uint64_t* tmem_full_bar = empty_bar + NS;      // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1;
-  const int npairs = gridDim.x >> 1;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < NS; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full_bar[b], 1);
-      mbar_init(&tmem_empty_bar[b], 8);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 0 && lane == 0) {
-    for (int v = 0; v < 3 * kMaxViews; ++v) tma_prefetch_desc(&p.maps[v]);
-  }
-  if (warp == 1) tmem_alloc_2sm(tmem_slot, 512);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  // unit -> (I, J) of the 256-column tile pair, split
-  auto decode = [&](int u, int& I, int& J, int& split) {
-    int t = u % p.ntiles;
-    split = u / p.ntiles;
-    int rowlen = p.nb2;
-    I = 0;
-    while (t >= rowlen) { t -= rowlen; ++I; --rowlen; }
-    J = I + t;
   };
 
-  if (warp == 0) {
-    // ================= TMA producer (both CTAs, each loads its own halves) =================
-    if (elect_one()) {
-      const uint32_t bytes_pair = 2u * Cfg::kStage;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int u = pair; u < p.total_units; u += npairs) {
-        int I, J, split;
-        decode(u, I, J, split);
-        const int blkA = min(2 * I + (int)rank, p.nblocks);
-        const int blkB = min(2 * J + (int)rank, p.nblocks);
-        const int vA = p.blk_view[blkA], colA = p.blk_col0[blkA];
-        const int vB = p.blk_view[blkB], colB = p.blk_col0[blkB];
-        const int c0 = split * p.chunks_per_split;
-        const int c1 = min(c0 + p.chunks_per_split, p.total_chunks);
-        for (int c = c0; c < c1; ++c) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (leader) mbar_arrive_expect_tx(&full_bar[stage], bytes_pair);
-          uint8_t* st = smem + stage * Cfg::kStage;
-          const int row = c * KC;
+  float acc[64];
 #pragma unroll
-          for (int a = 0; a < 4; ++a)
-            tma_load_2d_2sm(st + a * Cfg::kAtom, &p.maps[vA], &full_bar[stage], colA + 32 * a, row);
-#pragma unroll
-          for (int a = 0; a < 4; ++a)
-            tma_load_2d_2sm(st + (4 + a) * Cfg::kAtom, &p.maps[vB], &full_bar[stage], colB + 32 * a, row);
-          uint8_t* bf = st + Cfg::kRaw;
-#pragma unroll
-          for (int o = 0; o < 2; ++o) {      // 0: bhi, 1: blo
-#pragma unroll
-            for (int a = 0; a < 2; ++a) {
-              tma_load_2d_2sm(bf + (o * 2 + a) * Cfg::kAtom, &p.maps[(1 + o) * kMaxViews + vA], &full_bar[stage],
-                              colA + 64 * a, row);
-              tma_load_2d_2sm(bf + (4 + o * 2 + a) * Cfg::kAtom, &p.maps[(1 + o) * kMaxViews + vB], &full_bar[stage],
-                              colB + 64 * a, row);
-            }
-          }
-          if (++stage == NS) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer: one thread of the LEADER CTA drives both SMs =================
-    if (leader) {
-      const uint32_t idesc_tf = umma_idesc_tf32_mn(256, 256);
-      const uint32_t idesc_bf = umma_idesc_bf16_mn(256, 256);
-      const uint32_t sb = smem_u32(smem);
-      const uint64_t dA_tf = umma_smem_desc(sb, KC * 128, 512, kUmmaLayout);
-      const uint64_t dB_tf = umma_smem_desc(sb + 4 * Cfg::kAtom, KC * 128, 512, kUmmaLayout);
-      const uint64_t dA_bhi = umma_smem_desc(sb + Cfg::kRaw, KC * 128, 1024, 2);
-      const uint64_t dA_blo = umma_smem_desc(sb + Cfg::kRaw + Cfg::kBf, KC * 128, 1024, 2);
-      const uint64_t dB_bhi = umma_smem_desc(sb + Cfg::kRaw + 2 * Cfg::kBf, KC * 128, 1024, 2);
-      const uint64_t dB_blo = umma_smem_desc(sb + Cfg::kRaw + 3 * Cfg::kBf, KC * 128, 1024, 2);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int u = pair; u < p.total_units; u += npairs, ++it) {
-        const int split = u / p.ntiles;
-        const int c0 = split * p.chunks_per_split;
-        const int c1 = min(c0 + p.chunks_per_split, p.total_chunks);
-        const uint32_t b = (uint32_t)it & 1u, use = (uint32_t)it >> 1;
-        mbar_wait(&tmem_empty_bar[b], (use & 1u) ^ 1u);   // accumulator b drained by both CTAs' epilogue warps
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + b * 256u;
-        uint32_t acc = 0u;
-        for (int c = c0; c < c1; ++c) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint64_t so = (uint64_t)((stage * Cfg::kStage) >> 4);
-            umma_f16_2sm(tacc, dA_blo + so, dB_bhi + so, idesc_bf, acc);
-            umma_f16_2sm(tacc, dA_bhi + so, dB_blo + so, idesc_bf, 1u);
-            umma_tf32_2sm(tacc, dA_tf + so, dB_tf + so, idesc_tf, 1u);
-            umma_tf32_2sm(tacc, dA_tf + so + 64, dB_tf + so + 64, idesc_tf, 1u);
-            umma_commit_2sm(&empty_bar[stage], 3);
-          }
-          acc = 1u;
-          __syncwarp();
-          if (++stage == NS) { stage = 0; phase ^= 1; }
-        }
-        if (elect_one()) umma_commit_2sm(&tmem_full_bar[b], 3);
-        __syncwarp();
-      }
-    }
-  } else {
-    // ================= epilogue (both CTAs): own 128 accumulator rows x 256 columns per unit =================
-    const int g = warp & 3;
-    const int m = g * 32 + lane;
-    int it = 0;
-    for (int u = pair; u < p.total_units; u += npairs, ++it) {
-      int I, J, split;
-      decode(u, I, J, split);
-      const uint32_t b = (uint32_t)it & 1u, use = (uint32_t)it >> 1;
-      const size_t prow_idx = (size_t)(2 * I + rank) * 128 + m;
-      float* prow = p.partial + ((size_t)split * p.Dp2 + prow_idx) * p.Dp2;
-      mbar_wait(&tmem_full_bar[b], use & 1u);
-      tc_fence_after();
-      const uint32_t tacc = tmem_base + ((uint32_t)(g * 32) << 16) + b * 256u;
-#pragma unroll 1
-      for (int cc = 0; cc < 8; ++cc) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tacc + cc * 32, r);
-        tmem_ld_wait();
-        float4* dst = reinterpret_cast<float4*>(prow + (size_t)(2 * J + (cc >> 2)) * 128 + (cc & 3) * 32);
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          dst[q] = make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]),
-                               __uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3]));
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tmem_empty_bar[b], 0u);
-    }
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  const int wg = threadIdx.x >> 7;
+  if (nch > 0) {
+    load(0);
+    store(0);
   }
-
-  tc_fence_before();
-  cluster_sync_all();  // nobody frees TMEM / exits while the pair is still using either CTA's resources
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, 512);
-  }
-}
-
-// pre-pass of the persistent kernel: the bf16 copies of tf32_bf16_split_kernel AND the exact fp32 column sums of a slab of
-// rows per block (psum[slab][padded column], pad columns written as zero; summed in fixed order by reduce_colsums_kernel)
-template <int VEC>
-__global__ void __launch_bounds__(256)   // blockDim.x columns-groups (<= 256) of VEC columns, one slab of rows
-tf32_bf16_split_sums_kernel(const float* __restrict__ x, int64_t n, int d, int64_t ldx, uint16_t* __restrict__ bhi,
-                            uint16_t* __restrict__ blo, int64_t ldo, int rows_per_slab, float* __restrict__ psum,
-                            int ldps, int pw) {
-  const int c = (blockIdx.x * blockDim.x + threadIdx.x) * VEC;
-  if (c >= pw) return;
-  const int64_t r0 = (int64_t)blockIdx.y * rows_per_slab;
-  const int64_t r1 = r0 + rows_per_slab < n ? r0 + rows_per_slab : n;
-  float acc[VEC];
-#pragma unroll
-  for (int q = 0; q < VEC; ++q) acc[q] = 0.f;
-  if (c < d) {
-    if (VEC == 4) {
-#pragma unroll 4
-      for (int64_t r = r0; r < r1; ++r) {
-        const float4 v = *reinterpret_cast<const float4*>(x + r * ldx + c);
-        const float vv[4] = {v.x, v.y, v.z, v.w};
-        uint32_t h[4], l[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float hi = __uint_as_float(__float_as_uint(vv[q]) & 0xFFFFE000u);
-          h[q] = bf16_rn_bits(hi);
-          l[q] = bf16_rn_bits(vv[q] - hi);
-          acc[q % VEC] += vv[q];
-        }
-        *reinterpret_cast<uint2*>(bhi + r * ldo + c) = make_uint2(h[0] | (h[1] << 16), h[2] | (h[3] << 16));
-        *reinterpret_cast<uint2*>(blo + r * ldo + c) = make_uint2(l[0] | (l[1] << 16), l[2] | (l[3] << 16));
-      }
-    } else {
-#pragma unroll 4
-      for (int64_t r = r0; r < r1; ++r) {
-        const float v = x[r * ldx + c];
-        const float hi = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
-        bhi[r * ldo + c] = (uint16_t)bf16_rn_bits(hi);
-        blo[r * ldo + c] = (uint16_t)bf16_rn_bits(v - hi);
-        acc[0] += v;
-      }
-    }
-  }
-#pragma unroll
-  for (int q = 0; q < VEC; ++q) psum[(size_t)blockIdx.y * ldps + c + q] = acc[q];
-}
-
-// out[col] = sum over the S slabs of psum[s][col] in double, fixed order (32 strided chains, then a 32-term tail)
-__global__ void __launch_bounds__(1024)
-reduce_colsums_kernel(const float* __restrict__ psum, int S, int ldps, int Dp, double* __restrict__ out,
-                      int accumulate) {
-  __shared__ double sm[32][33];
-  const int cx = threadIdx.x & 31, g = threadIdx.x >> 5;
-  const int col = blockIdx.x * 32 + cx;
-  double acc = 0.0;
-  if (col < Dp)
-    for (int s = g; s < S; s += 32) acc += (double)psum[(size_t)s * ldps + col];
-  sm[g][cx] = acc;
+  fence_proxy_async_smem();
   __syncthreads();
-  if (g == 0 && col < Dp) {
-    double t = 0.0;
+  for (int c = 0; c < nch; ++c) {
+    const uint32_t st = smem_u32(smem + (c & 1) * Cfg::kStage);
+    const uint32_t a0 = st + wg * 64 * 128;                       // this warpgroup's 64 rows of the A tile
+    const uint32_t b0 = diag ? st : st + Cfg::kOps * kWgTile;     // a diagonal tile multiplies A by itself
+    wgmma_fence();
 #pragma unroll
-    for (int i = 0; i < 32; ++i) t += sm[i][cx];
-    out[col] = accumulate ? out[col] + t : t;
-  }
-}
-
-
-// 3xTF32 operand split.  The tensor core TRUNCATES its fp32 operands to TF32 (measured: tools/probe_trunc.py),
-// so the raw array itself serves as the "hi" operand (hi = x with the low 13 mantissa bits cleared) and only
-// the residual lo = rna_tf32(x - hi) is materialised (exact subtraction, then 11 significant bits: the
-// hardware's own truncation of lo is a no-op).  x = hi + lo + O(2^-21 |x|).  One HBM-bound pre-pass:
-// reads n*d*4 bytes, writes n*d*4 bytes.
-// round-to-nearest variant: hi = rna_tf32(x), lo = rna_tf32(x - hi); both operands materialised
-__global__ void tf32_split_rn_kernel(const float* __restrict__ x, int64_t n, int d, int64_t ldx,
-                                     float* __restrict__ hi, float* __restrict__ lo, int64_t ldo) {
-  const int64_t total = n * (int64_t)d;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t r = i / d;
-    const int c = (int)(i - r * d);
-    const float v = x[r * ldx + c];
-    uint32_t h;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(v));
-    const float hf = __uint_as_float(h);
-    uint32_t l;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(v - hf));
-    hi[r * ldo + c] = hf;
-    lo[r * ldo + c] = __uint_as_float(l);
-  }
-}
-
-__global__ void tf32_residual_kernel(const float* __restrict__ x, int64_t n, int d, int64_t ldx,
-                                     float* __restrict__ lo, int64_t ldo, int vec4) {
-  if (vec4) {
-    const int d4 = d >> 2;
-    const int64_t total = n * (int64_t)d4;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
-         i += (int64_t)gridDim.x * blockDim.x) {
-      const int64_t r = i / d4;
-      const int c = (int)(i - r * d4) << 2;
-      const float4 v = *reinterpret_cast<const float4*>(x + r * ldx + c);
-      float4 o;
-      o.x = tf32_residual(v.x);
-      o.y = tf32_residual(v.y);
-      o.z = tf32_residual(v.z);
-      o.w = tf32_residual(v.w);
-      *reinterpret_cast<float4*>(lo + r * ldo + c) = o;
+    for (int kk = 0; kk < kWgKC / 8; ++kk) {
+      const uint64_t a_hi = wgmma_desc_k128(a0 + 32 * kk), b_hi = wgmma_desc_k128(b0 + 32 * kk);
+      if (X3) {
+        const uint64_t a_lo = wgmma_desc_k128(a0 + kWgTile + 32 * kk), b_lo = wgmma_desc_k128(b0 + kWgTile + 32 * kk);
+        wgmma_tf32<128>(acc, a_lo, b_hi);   // small cross terms first
+        wgmma_tf32<128>(acc, a_hi, b_lo);
+      }
+      wgmma_tf32<128>(acc, a_hi, b_hi);
     }
-  } else {
-    const int64_t total = n * (int64_t)d;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
-         i += (int64_t)gridDim.x * blockDim.x) {
-      const int64_t r = i / d;
-      const int c = (int)(i - r * d);
-      lo[r * ldo + c] = tf32_residual(x[r * ldx + c]);
-    }
+    wgmma_commit();
+    const bool more = c + 1 < nch;
+    if (more) load(c + 1);
+    wgmma_wait_all();
+    wgmma_fence_regs<64>(acc);
+    if (more) store((c + 1) & 1);   // that stage was last read by the wgmmas of slice c - 1, retired before the barrier
+    fence_proxy_async_smem();
+    __syncthreads();
+  }
+
+  // ---- epilogue: fragments -> partial slab of this split ----
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  float* P = p.partial + (size_t)split * p.Dp * p.Dp;
+  const int row0 = bi * kBlk + wg * 64 + warp * 16 + (lane >> 2);
+  const int col0 = bj * kBlk + 2 * (lane & 3);
+#pragma unroll
+  for (int r = 0; r < 64; r += 2) {
+    const int row = row0 + 8 * ((r >> 1) & 1), col = col0 + 8 * (r >> 2);
+    *reinterpret_cast<float2*>(P + (size_t)row * p.Dp + col) = make_float2(acc[r], acc[r + 1]);
+  }
+  if (diag) {
+    if (threadIdx.x >= kBlk) colsum_hi[threadIdx.x - kBlk] = csum;
+    __syncthreads();
+    if (threadIdx.x < kBlk)
+      p.partial_sum[(size_t)split * p.Dp + bi * kBlk + threadIdx.x] = csum + colsum_hi[threadIdx.x];
   }
 }
-
 // =============================================================================================
 // exact SIMT kernel (fp32 / fp64), 64x64 tiles inside the same padded tile space
 // =============================================================================================
@@ -1124,7 +285,7 @@ __global__ void __launch_bounds__(256) moments_simt_kernel(const SimtParams p) {
 }
 
 // =============================================================================================
-// fp64 tensor-core variant of the exact kernel: mma.sync.aligned.m8n8k4.row.col.f64 (DMMA; tcgen05 has no
+// fp64 tensor-core variant of the exact kernel: mma.sync.aligned.m8n8k4.row.col.f64 (DMMA; wgmma has no
 // f64 kind).  Same 64x64 tiles, same partial layout and split planning as moments_simt_kernel<double>.
 // 8 warps; warp w owns the 32 x 16 sub-tile (rows 32*(w&1), cols 16*(w>>1)) = 4 x 2 m8n8 fragments.
 // Shared tiles are [k][64 + 8] doubles: the 16-bank skew between consecutive k rows makes the 64-bit
@@ -1300,150 +461,49 @@ __global__ void covariance_kernel(const CovParams p, const double* __restrict__ 
 // =============================================================================================
 namespace {
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                  CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(f);
-  });
-  return fn;
-}
-
-int encode_view_map(CUtensorMap* map, const void* ptr, int64_t n_rows, int64_t d, int64_t ld, int kc) {
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled entry point not available (driver too old?)");
-    return -2;
-  }
-  CCAB_CHECK_ARG((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "view pointer must be 16-byte aligned for TMA");
-  CCAB_CHECK_ARG((ld * 4) % 16 == 0, "leading dimension (%lld floats) must be a multiple of 4 for TMA",
-                 (long long)ld);
-  cuuint64_t gdim[2] = {(cuuint64_t)d, (cuuint64_t)n_rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)ld * 4};
-  cuuint32_t box[2] = {32, (cuuint32_t)kc};
-  cuuint32_t estr[2] = {1, 1};
-  CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  if (tc_debug().tma_dtype >= 0) dt = (CUtensorMapDataType)tc_debug().tma_dtype;
-  CUresult r = enc(map, dt, 2, const_cast<void*>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed with CUresult %d (d=%lld n=%lld ld=%lld)", (int)r, (long long)d,
-              (long long)n_rows, (long long)ld);
-    return -3;
-  }
-  return 0;
-}
-
-int encode_bf16_map(CUtensorMap* map, const void* ptr, int64_t n_rows, int64_t d, int64_t ld, int kc) {
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled entry point not available (driver too old?)");
-    return -2;
-  }
-  cuuint64_t gdim[2] = {(cuuint64_t)d, (cuuint64_t)n_rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)kc};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled (bf16) failed with CUresult %d (d=%lld n=%lld ld=%lld)", (int)r, (long long)d,
-              (long long)n_rows, (long long)ld);
-    return -3;
-  }
-  return 0;
-}
-
 int sm_count() {
   static int n[64] = {};   // per device ordinal (a process may drive several GPUs)
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return 148;
+  if (dev < 0 || dev >= 64) return 132;
   if (!n[dev]) {
     cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (n[dev] <= 0) n[dev] = 148;
+    if (n[dev] <= 0) n[dev] = 132;
   }
   return n[dev];
 }
 
 struct TcPlan {
-  int kc, total_chunks, num_splits, chunks_per_split, ntiles;
-  int two_cta, nb2, ldp;  // ldp: leading dimension of the partial slabs (Dp, or nb2*256 for the CTA-pair kernel)
-  int sum_rows, sum_slabs;  // tf32x3b: rows per block / number of column-sum slabs of the pre-pass
-  size_t partial_bytes, sum_bytes, split_bytes;  // split_bytes: hi/lo operand copies (3xTF32)
+  int total_chunks, num_splits, chunks_per_split, ntiles;
+  size_t partial_bytes, sum_bytes;
 };
 
 TcPlan plan_tc(const ColumnLayout& L, int64_t n_rows, int mode) {
-  const bool x3 = mode != 0;   // 0: one TF32 pass, 1: 3xTF32, 3: 3xTF32 with bf16 cross terms
+  const bool x3 = mode != 0;   // 0: one TF32 pass, 1 and 3: 3xTF32
   TcPlan P;
-  P.kc = x3 ? 16 : 32;
-  if (!x3 && tc_debug().variant != 1 && (tc_debug().kc == 16 || tc_debug().kc == 64)) P.kc = tc_debug().kc;
-  P.total_chunks = (int)ceil_div(n_rows, P.kc);
-  P.two_cta = tc_debug().variant != 1 || mode == 3;
-  P.nb2 = (L.nblocks + 1) / 2;
-  int nt = 0;
-  if (P.two_cta) {
-    nt = P.nb2 * (P.nb2 + 1) / 2;
-    P.ldp = P.nb2 * 256;
-  } else {
-    for (int i = 0; i < L.nblocks; ++i) nt += (L.nblocks - i + 1) / 2;
-    P.ldp = L.Dp;
-  }
-  P.ntiles = nt;
-  const int slots = P.two_cta ? sm_count() / 2 : sm_count();  // CTA pairs occupy two SMs
-  int S = 1;
+  P.total_chunks = (int)ceil_div(n_rows, kWgKC);
+  P.ntiles = L.nblocks * (L.nblocks + 1) / 2;
+  // about four waves of CTAs, so that the tile count does not leave a mostly idle last wave
+  int S = (int)ceil_div(4 * sm_count(), P.ntiles);
   int max_splits = 64;
-  if (nt < slots) S = slots / nt;
   if (x3) {
-    // tcgen05 accumulates in fp32 with round-toward-zero: a monotone sum (every diagonal entry of M) drifts
-    // low by ~0.5 ulp per accumulation step -- measured -1.4e-4 relative on the diagonal for 8192-sample runs,
-    // uniform to 1e-6 (tools/probe_x3.py), which acts like a negative ridge and costs ~1e-3 in the weights.
-    // The 3xTF32 mode exists for fp32-grade results, so bound one accumulator run to 2048 samples (256 k-steps,
-    // drift < 4e-5) and let the fixed-order double reduction of the partials do the long sum.  Measured cost
-    // of 49 instead of 2 splits at n=1e5: none (tools/probe_x3b.py).
+    // The 3xTF32 mode exists for fp32-grade results: one fp32 accumulator run is bounded to 2048 samples and the
+    // fixed-order float64 reduction of the split partials does the long sum.
     S = std::max<int64_t>(S, ceil_div(n_rows, 2048));
     max_splits = 256;
   }
-  const int min_chunks = 8;  // keep the pipeline prologue/epilogue amortised
+  const int min_chunks = 8;  // keep the per-CTA prologue / epilogue amortised
   S = (int)std::min<int64_t>(S, std::max<int64_t>(1, P.total_chunks / min_chunks));
   // keep the split partials below 2 GiB
-  const int64_t slab = (int64_t)P.ldp * P.ldp * (int64_t)sizeof(float);
+  const int64_t slab = (int64_t)L.Dp * L.Dp * (int64_t)sizeof(float);
   max_splits = (int)std::max<int64_t>(1, std::min<int64_t>(max_splits, ((int64_t)2 << 30) / slab));
   S = std::min(S, max_splits);
   if (tc_debug().force_splits > 0) S = tc_debug().force_splits;
   S = std::max(1, std::min(S, P.total_chunks));
   P.chunks_per_split = (int)ceil_div(P.total_chunks, S);
   P.num_splits = (int)ceil_div(P.total_chunks, P.chunks_per_split);
-  P.partial_bytes = (size_t)P.num_splits * P.ldp * P.ldp * sizeof(float);
-  P.sum_bytes = (size_t)P.num_splits * P.ldp * sizeof(float);
-  P.split_bytes = 0;
-  P.sum_rows = P.sum_slabs = 0;
-  if (mode == 3) {
-    P.sum_rows = (int)std::max<int64_t>(8, ceil_div(ceil_div(n_rows, 1024), 8) * 8);   // <= 1024 slabs, >= 8 rows each
-    P.sum_slabs = (int)ceil_div(n_rows, P.sum_rows);
-    P.sum_bytes = (size_t)std::max(P.num_splits, P.sum_slabs) * P.ldp * sizeof(float);
-    for (int v = 0; v < L.n_views; ++v) {
-      int64_t ldo = ceil_div(L.dims[v], 8) * 8;
-      P.split_bytes += 2 * (size_t)n_rows * ldo * sizeof(uint16_t) + 512;   // bhi + blo
-    }
-  } else if (x3) {
-    for (int v = 0; v < L.n_views; ++v) {
-      int64_t ldo = ceil_div(L.dims[v], 4) * 4;
-      // lo only; hi as well for the round-to-nearest split (debug)
-      P.split_bytes += (tc_debug().x3_split == 1 ? 2 : 1) * (size_t)n_rows * ldo * sizeof(float);
-    }
-  }
+  P.partial_bytes = (size_t)P.num_splits * L.Dp * L.Dp * sizeof(float);
+  P.sum_bytes = (size_t)P.num_splits * L.Dp * sizeof(float);
   return P;
 }
 
@@ -1451,8 +511,7 @@ TcPlan plan_tc(const ColumnLayout& L, int64_t n_rows, int mode) {
 // 2048-sample accumulator run
 int64_t tc_rows_cap(const ColumnLayout& L, int mode) {
   if (mode == 0) return (int64_t)1 << 31;
-  const int64_t ldp = (tc_debug().variant != 1 || mode == 3) ? (int64_t)((L.nblocks + 1) / 2) * 256 : L.Dp;
-  const int64_t slab = ldp * ldp * (int64_t)sizeof(float);
+  const int64_t slab = (int64_t)L.Dp * L.Dp * (int64_t)sizeof(float);
   const int64_t max_splits = std::max<int64_t>(1, std::min<int64_t>(256, ((int64_t)2 << 30) / slab));
   return max_splits * 2048;
 }
@@ -1486,7 +545,7 @@ size_t moments_workspace_bytes(int dtype, int precision, const ColumnLayout& L, 
     return align256((size_t)P.num_splits * L.Dp * L.Dp * el) + align256((size_t)P.num_splits * L.Dp * el);
   }
   TcPlan P = plan_tc(L, std::min(n_rows, tc_rows_cap(L, precision)), precision);   // sized for one pass
-  return align256(P.partial_bytes) + align256(P.sum_bytes) + align256(P.split_bytes) + 256;
+  return align256(P.partial_bytes) + align256(P.sum_bytes) + 256;
 }
 
 namespace {
@@ -1523,266 +582,45 @@ int moments_tf32(const ColumnLayout& L, const void* const* views, const int64_t*
 namespace {
 int moments_tf32_pass(const ColumnLayout& L, const void* const* views, const int64_t* lds, int64_t n_rows, int mode,
                       double* moments_out, void* ws, size_t ws_bytes, cudaStream_t stream, int accumulate) {
-  const bool x3 = mode == 1;
   TcPlan P = plan_tc(L, n_rows, mode);
-  const size_t need = align256(P.partial_bytes) + align256(P.sum_bytes) + align256(P.split_bytes) + 256;
+  const size_t need = align256(P.partial_bytes) + align256(P.sum_bytes) + 256;
   CCAB_CHECK_ARG(ws_bytes >= need, "workspace too small: %zu < %zu", ws_bytes, need);
   uint8_t* w = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
-
   float* d_partial = reinterpret_cast<float*>(w);
   float* d_partial_sum = reinterpret_cast<float*>(w + align256(P.partial_bytes));
-  uint8_t* splitbuf = w + align256(P.partial_bytes) + align256(P.sum_bytes);
 
-  if (mode == 3) {
-    // ---- 3xTF32 with bf16 cross terms: raw view (tf32 hi by truncation) + bf16 copies of hi and lo ----
-    TcParams3 prm;
-    memset(&prm, 0, sizeof(prm));
-    const bool persist = tc_debug().x3b_oneshot == 0;
-    for (int v = 0; v < L.n_views; ++v) {
-      const float* x = static_cast<const float*>(views[v]);
-      const int64_t ldo = ceil_div(L.dims[v], 8) * 8;
-      uint16_t* bhi = reinterpret_cast<uint16_t*>(splitbuf);
-      uint16_t* blo = bhi + (size_t)n_rows * ldo;
-      splitbuf += align256(2 * (size_t)n_rows * ldo * sizeof(uint16_t));
-      const int vec4 = (L.dims[v] % 4 == 0) && (lds[v] % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0);
-      if (persist) {
-        const int pw = L.poff[v + 1] - L.poff[v];   // padded width of this view (multiple of 128)
-        float* ps = d_partial_sum + L.poff[v];
-        if (vec4) {
-          const int bt = std::min(256, pw / 4);          // pw is a multiple of 128: 32 .. 256 threads, none idle
-          dim3 grid((unsigned)ceil_div(pw, 4 * bt), (unsigned)P.sum_slabs);
-          tf32_bf16_split_sums_kernel<4><<<grid, bt, 0, stream>>>(x, n_rows, L.dims[v], lds[v], bhi, blo, ldo, P.sum_rows,
-                                                                 ps, P.ldp, pw);
-        } else {
-          const int bt = std::min(256, pw);
-          dim3 grid((unsigned)ceil_div(pw, bt), (unsigned)P.sum_slabs);
-          tf32_bf16_split_sums_kernel<1><<<grid, bt, 0, stream>>>(x, n_rows, L.dims[v], lds[v], bhi, blo, ldo, P.sum_rows,
-                                                                 ps, P.ldp, pw);
-        }
-      } else {
-        const int64_t total = n_rows * (int64_t)L.dims[v] / (vec4 ? 4 : 1);
-        int blocks = (int)std::min<int64_t>(ceil_div(total, 256), (int64_t)sm_count() * 16);
-        tf32_bf16_split_kernel<<<blocks, 256, 0, stream>>>(x, n_rows, L.dims[v], lds[v], bhi, blo, ldo, vec4);
-      }
-      count_launches(1);
-      CCAB_CUDA(cudaGetLastError());
-      int rc = encode_view_map(&prm.maps[v], x, n_rows, L.dims[v], lds[v], P.kc);
-      if (rc) return rc;
-      rc = encode_bf16_map(&prm.maps[kMaxViews + v], bhi, n_rows, L.dims[v], ldo, P.kc);
-      if (rc) return rc;
-      rc = encode_bf16_map(&prm.maps[2 * kMaxViews + v], blo, n_rows, L.dims[v], ldo, P.kc);
-      if (rc) return rc;
-    }
-    for (int v = L.n_views; v < kMaxViews; ++v) {
-      prm.maps[v] = prm.maps[0];
-      prm.maps[kMaxViews + v] = prm.maps[kMaxViews];
-      prm.maps[2 * kMaxViews + v] = prm.maps[2 * kMaxViews];
-    }
-    prm.partial = d_partial;
-    prm.partial_sum = d_partial_sum;
-    prm.total_chunks = P.total_chunks;
-    prm.chunks_per_split = P.chunks_per_split;
-    prm.num_splits = P.num_splits;
-    prm.nblocks = L.nblocks;
-    prm.nb2 = P.nb2;
-    prm.Dp2 = P.ldp;
-    int b = 0;
-    for (int v = 0; v < L.n_views; ++v)
-      for (int c = 0; c < L.dims[v]; c += kBlk, ++b) {
-        prm.blk_view[b] = (uint8_t)v;
-        prm.blk_col0[b] = c;
-      }
-    for (; b < kMaxBlocks + 2; ++b) {
-      prm.blk_view[b] = 0;
-      prm.blk_col0[b] = 1 << 30;
-    }
-    prm.ntiles = P.ntiles;
-    prm.total_units = P.ntiles * P.num_splits;
-    using Cfg = Tc3Cfg<6>;
-    static bool attr_done[64] = {};
-    static int max_pairs[64] = {};
-    int dev = 0;
-    CCAB_CUDA(cudaGetDevice(&dev));
-    const int di = (dev >= 0 && dev < 64) ? dev : 0;
-    if (dev < 0 || dev >= 64 || !attr_done[dev]) {
-      CCAB_CUDA(cudaFuncSetAttribute(moments_x3b_2cta_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-      CCAB_CUDA(cudaFuncSetAttribute(moments_x3b_persist_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     Cfg::kSmem));
-      // how many CTA pairs are co-resident (GPCs with an odd number of free SMs cannot host a pair)
-      cudaLaunchConfig_t cfg;
-      memset(&cfg, 0, sizeof(cfg));
-      cfg.gridDim = dim3(2 * (unsigned)(sm_count() / 2));
-      cfg.blockDim = dim3(kTcThreads);
-      cfg.dynamicSmemBytes = Cfg::kSmem;
-      cudaLaunchAttribute at;
-      memset(&at, 0, sizeof(at));
-      at.id = cudaLaunchAttributeClusterDimension;
-      at.val.clusterDim.x = 2;
-      at.val.clusterDim.y = 1;
-      at.val.clusterDim.z = 1;
-      cfg.attrs = &at;
-      cfg.numAttrs = 1;
-      int nc = 0;
-      if (cudaOccupancyMaxActiveClusters(&nc, moments_x3b_persist_kernel<6>, &cfg) != cudaSuccess || nc <= 0) {
-        cudaGetLastError();
-        nc = sm_count() / 2;
-      }
-      max_pairs[di] = std::min(nc, sm_count() / 2);
-      if (dev >= 0 && dev < 64) attr_done[dev] = true;
-    }
-    if (g_prof_on) cudaEventRecord(g_prof_e0, stream);
-    if (persist) {
-      const int npairs = std::max(1, std::min(max_pairs[di], prm.total_units));
-      moments_x3b_persist_kernel<6><<<dim3(2 * npairs), kTcThreads, Cfg::kSmem, stream>>>(prm);
-    } else {
-      moments_x3b_2cta_kernel<6><<<dim3(2 * P.ntiles, P.num_splits), kTcThreads, Cfg::kSmem, stream>>>(prm);
-    }
-    count_launches(1);
-    CCAB_CUDA(cudaGetLastError());
-    if (g_prof_on) {
-      cudaEventRecord(g_prof_e1, stream);
-      g_prof_valid = true;
-    }
-    const size_t total = (size_t)L.Dp * L.Dp + (persist ? 0 : L.Dp);
-    int rblocks = (int)std::min<size_t>((total + 255) / 256, (size_t)sm_count() * 8);
-    reduce_partials_kernel<float><<<rblocks, 256, 0, stream>>>(d_partial, persist ? nullptr : d_partial_sum, P.num_splits,
-                                                              L.Dp, P.ldp, kBlk, moments_out, accumulate);
-    count_launches(1);
-    CCAB_CUDA(cudaGetLastError());
-    if (persist) {
-      reduce_colsums_kernel<<<(unsigned)ceil_div(L.Dp, 32), 1024, 0, stream>>>(d_partial_sum, P.sum_slabs, P.ldp, L.Dp,
-                                                                             moments_out + (size_t)L.Dp * L.Dp, accumulate);
-      count_launches(1);
-      CCAB_CUDA(cudaGetLastError());
-    }
-    return 0;
-  }
-
-  // operands (raw, or hi/lo copies for 3xTF32) and their tensor maps
-  CUtensorMap maps[2 * kMaxViews];
+  WgParams prm;
+  memset(&prm, 0, sizeof(prm));
   for (int v = 0; v < L.n_views; ++v) {
-    const float* x = static_cast<const float*>(views[v]);
-    if (x3 && tc_debug().x3_split == 1) {
-      const int64_t ldo = ceil_div(L.dims[v], 4) * 4;
-      float* hi = reinterpret_cast<float*>(splitbuf);
-      float* lo = hi + (size_t)n_rows * ldo;
-      splitbuf += 2 * (size_t)n_rows * ldo * sizeof(float);
-      const int64_t total = n_rows * (int64_t)L.dims[v];
-      int blocks = (int)std::min<int64_t>(ceil_div(total, 256), (int64_t)sm_count() * 16);
-      tf32_split_rn_kernel<<<blocks, 256, 0, stream>>>(x, n_rows, L.dims[v], lds[v], hi, lo, ldo); count_launches(1);
-      CCAB_CUDA(cudaGetLastError());
-      int rc = encode_view_map(&maps[v], hi, n_rows, L.dims[v], ldo, P.kc);
-      if (rc) return rc;
-      rc = encode_view_map(&maps[kMaxViews + v], lo, n_rows, L.dims[v], ldo, P.kc);
-      if (rc) return rc;
-    } else if (x3) {
-      const int64_t ldo = ceil_div(L.dims[v], 4) * 4;
-      float* lo = reinterpret_cast<float*>(splitbuf);
-      splitbuf += (size_t)n_rows * ldo * sizeof(float);
-      const int vec4 = (L.dims[v] % 4 == 0) && (lds[v] % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0);
-      const int64_t total = n_rows * (int64_t)L.dims[v] / (vec4 ? 4 : 1);
-      int blocks = (int)std::min<int64_t>(ceil_div(total, 256), (int64_t)sm_count() * 16);
-      tf32_residual_kernel<<<blocks, 256, 0, stream>>>(x, n_rows, L.dims[v], lds[v], lo, ldo, vec4); count_launches(1);
-      CCAB_CUDA(cudaGetLastError());
-      int rc = encode_view_map(&maps[v], x, n_rows, L.dims[v], lds[v], P.kc);   // "hi" = the raw view (HW truncates)
-      if (rc) return rc;
-      rc = encode_view_map(&maps[kMaxViews + v], lo, n_rows, L.dims[v], ldo, P.kc);
-      if (rc) return rc;
-    } else {
-      int rc = encode_view_map(&maps[v], x, n_rows, L.dims[v], lds[v], P.kc);
-      if (rc) return rc;
-      maps[kMaxViews + v] = maps[v];
+    prm.view_ptr[v] = static_cast<const float*>(views[v]);
+    prm.view_ld[v] = lds[v];
+    prm.view_dim[v] = L.dims[v];
+  }
+  int b = 0;
+  for (int v = 0; v < L.n_views; ++v)
+    for (int c = 0; c < L.dims[v]; c += kBlk, ++b) {
+      prm.blk_view[b] = (uint8_t)v;
+      prm.blk_col0[b] = c;
     }
-  }
-  for (int v = L.n_views; v < kMaxViews; ++v) {
-    maps[v] = maps[0];
-    maps[kMaxViews + v] = maps[kMaxViews];
-  }
-  const int lbo = tc_debug().lbo_bytes >= 0 ? tc_debug().lbo_bytes : P.kc * 128;
-  const int sbo = tc_debug().sbo_bytes >= 0 ? tc_debug().sbo_bytes : 512;
-
+  prm.partial = d_partial;
+  prm.partial_sum = d_partial_sum;
+  prm.n_rows = n_rows;
+  prm.rows_per_split = (int64_t)P.chunks_per_split * kWgKC;
+  prm.nblocks = L.nblocks;
+  prm.Dp = L.Dp;
+  dim3 grid(P.ntiles, P.num_splits);
   if (g_prof_on) cudaEventRecord(g_prof_e0, stream);
-  if (P.two_cta) {
-    TcParams2 prm;
-    memset(&prm, 0, sizeof(prm));
-    memcpy(prm.maps, maps, sizeof(maps));
-    prm.partial = d_partial;
-    prm.partial_sum = d_partial_sum;
-    prm.total_chunks = P.total_chunks;
-    prm.chunks_per_split = P.chunks_per_split;
-    prm.num_splits = P.num_splits;
-    prm.nblocks = L.nblocks;
-    prm.nb2 = P.nb2;
-    prm.Dp2 = P.ldp;
-    prm.lbo_bytes = lbo;
-    prm.sbo_bytes = sbo;
-    int b = 0;
-    for (int v = 0; v < L.n_views; ++v)
-      for (int c = 0; c < L.dims[v]; c += kBlk, ++b) {
-        prm.blk_view[b] = (uint8_t)v;
-        prm.blk_col0[b] = c;
-      }
-    for (; b < kMaxBlocks + 2; ++b) {  // dummy blocks: every coordinate out of bounds -> TMA zero fill
-      prm.blk_view[b] = 0;
-      prm.blk_col0[b] = 1 << 30;
-    }
-    prm.dry_run = tc_debug().dry_run;
-    dim3 grid(2 * P.ntiles, P.num_splits);
-#define CCAB_LAUNCH_2CTA(KC_, X3_, NS_)                                                                      \
-  do {                                                                                                       \
-    using Cfg = Tc2Cfg<KC_, X3_, NS_>;                                                                       \
-    /* function attributes are per device / context: set on every call (ADVICE r1) */                       \
-    CCAB_CUDA(cudaFuncSetAttribute(moments_tf32_2cta_kernel<KC_, X3_, NS_>,                                  \
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));                \
-    moments_tf32_2cta_kernel<KC_, X3_, NS_><<<grid, kTcThreads, Cfg::kSmem, stream>>>(prm);                  \
-  } while (0)
-    if (x3) {
-      CCAB_LAUNCH_2CTA(16, true, 6);
-    } else if (P.kc == 64) {
-      CCAB_LAUNCH_2CTA(64, false, 3);
-    } else if (P.kc == 16) {
-      CCAB_LAUNCH_2CTA(16, false, 12);
-    } else {
-      CCAB_LAUNCH_2CTA(32, false, 6);
-    }
-#undef CCAB_LAUNCH_2CTA
-    count_launches(1);
+  if (mode != 0) {
+    // function attributes are per device / context: set on every call
+    CCAB_CUDA(cudaFuncSetAttribute(moments_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   WgCfg<true>::kSmem));
+    moments_wgmma_kernel<true><<<grid, kWgThreads, WgCfg<true>::kSmem, stream>>>(prm);
   } else {
-    TcParams prm;
-    memset(&prm, 0, sizeof(prm));
-    memcpy(prm.maps, maps, sizeof(maps));
-    prm.partial = d_partial;
-    prm.partial_sum = d_partial_sum;
-    prm.total_chunks = P.total_chunks;
-    prm.chunks_per_split = P.chunks_per_split;
-    prm.num_splits = P.num_splits;
-    prm.nblocks = L.nblocks;
-    prm.Dp = L.Dp;
-    prm.lbo_bytes = lbo;
-    prm.sbo_bytes = sbo;
-    int b = 0;
-    for (int v = 0; v < L.n_views; ++v)
-      for (int c = 0; c < L.dims[v]; c += kBlk, ++b) {
-        prm.blk_view[b] = (uint8_t)v;
-        prm.blk_col0[b] = c;
-      }
-    prm.row_tile_start[0] = 0;
-    for (int i = 0; i < L.nblocks; ++i) prm.row_tile_start[i + 1] = prm.row_tile_start[i] + (L.nblocks - i + 1) / 2;
-    for (int i = L.nblocks + 1; i <= kMaxBlocks; ++i) prm.row_tile_start[i] = 0x7fffffff;
-    dim3 grid(P.ntiles, P.num_splits);
-    if (x3) {
-      using Cfg = TcCfg<16, true>;
-      CCAB_CUDA(cudaFuncSetAttribute(moments_tf32_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     Cfg::kSmem));
-      moments_tf32_kernel<16, true><<<grid, kTcThreads, Cfg::kSmem, stream>>>(prm);
-    } else {
-      using Cfg = TcCfg<32, false>;
-      CCAB_CUDA(cudaFuncSetAttribute(moments_tf32_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     Cfg::kSmem));
-      moments_tf32_kernel<32, false><<<grid, kTcThreads, Cfg::kSmem, stream>>>(prm);
-    }
-    count_launches(1);
+    CCAB_CUDA(cudaFuncSetAttribute(moments_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   WgCfg<false>::kSmem));
+    moments_wgmma_kernel<false><<<grid, kWgThreads, WgCfg<false>::kSmem, stream>>>(prm);
   }
+  count_launches(1);
   CCAB_CUDA(cudaGetLastError());
   if (g_prof_on) {
     cudaEventRecord(g_prof_e1, stream);
@@ -1791,7 +629,7 @@ int moments_tf32_pass(const ColumnLayout& L, const void* const* views, const int
 
   const size_t total = (size_t)L.Dp * L.Dp + L.Dp;
   int rblocks = (int)std::min<size_t>((total + 255) / 256, (size_t)sm_count() * 8);
-  reduce_partials_kernel<float><<<rblocks, 256, 0, stream>>>(d_partial, d_partial_sum, P.num_splits, L.Dp, P.ldp,
+  reduce_partials_kernel<float><<<rblocks, 256, 0, stream>>>(d_partial, d_partial_sum, P.num_splits, L.Dp, L.Dp,
                                                             kBlk, moments_out, accumulate); count_launches(1);
   CCAB_CUDA(cudaGetLastError());
   return 0;

@@ -24,8 +24,9 @@ struct ColumnLayout {
 int make_layout(int n_views, const int64_t* dims, ColumnLayout* out);
 
 // --- launchers (all asynchronous on `stream`) -------------------------------------------------
-// precision: 0 = TF32 single pass (tcgen05), 1 = 3xTF32 split (tcgen05), 2 = exact SIMT FMA,
-//            3 = 3xTF32 with the two cross terms as bf16 MMAs (tcgen05 kind::f16).
+// precision: 0 = TF32 single pass (wgmma), 1 = 3xTF32 split (wgmma), 2 = exact SIMT FMA,
+//            3 = 3xTF32 (on Hopper the same kernel as 1; the bf16 cross-term variant needs a TF32 MMA that reads
+//            MN-major operands, which wgmma does not have).
 size_t moments_workspace_bytes(int dtype, int precision, const ColumnLayout& L, int64_t n_rows);
 
 int moments_tf32(const ColumnLayout& L, const void* const* views, const int64_t* lds, int64_t n_rows,
@@ -62,22 +63,14 @@ int moments_exchange_nvls(const ColumnLayout& L, double* moments, double n_local
                           double* sym_multicast, void* const* pads_dev, int rank, int world, int pad_slots,
                           int64_t sym_doubles, unsigned epoch, double* n_total_out, cudaStream_t stream);
 
-// debug knobs for the tcgen05 kernel (descriptor strides / TMA data type), see tools/umma_probe.py
+// debug knobs of the moment kernels
 struct TcDebug {
-  int lbo_bytes;    // <0: default
-  int sbo_bytes;    // <0: default
-  int tma_dtype;    // <0: default (FLOAT32); else a CUtensorMapDataType value
   int force_splits; // <=0: heuristic
-  int variant;      // 0: CTA-pair kernel (cta_group::2, default), 1: single-CTA kernel
-  int kc;           // CTA-pair kernel, 1-pass: rows per stage 16 / 32 (default) / 64
-  int dry_run;      // CTA-pair kernel: skip TMA after the first ring fill (MMA-rate experiment; wrong results)
-  int x3_split;     // 3xTF32 operand split: 0 = residual only (raw array is hi by truncation), 1 = round-to-nearest hi/lo
   int f64_simt;     // float64 inputs: 0 = DMMA kernel (default), 1 = CUDA-core FMA kernel
-  int x3b_oneshot;  // tf32x3b: 0 = persistent kernel, overlapped epilogue (default), 1 = one (tile, split) unit per CTA pair
 };
 TcDebug& tc_debug();
 
-// CUDA-event timing of the tcgen05 kernel launch alone (for bench.py's roofline line)
+// CUDA-event timing of the tensor-core moment kernel launch alone (for bench.py's roofline line)
 void moments_profile_enable(int on);
 float moments_profile_last_ms();
 

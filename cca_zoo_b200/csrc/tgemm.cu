@@ -1,41 +1,37 @@
-// tgemm: C = alpha * op(A) * op(B) + beta * C in fp32-grade arithmetic on the tcgen05 tensor cores.
+// tgemm: C = alpha * op(A) * op(B) + beta * C in fp32-grade arithmetic on the Hopper tensor cores (wgmma, 3xTF32).
 //
 // The solver stage after K1 (Cholesky panels and trailing updates, L^-1 assembly, T = L1^-1 C12 L2^-T, the
 // subspace iteration, the back-substitution of the weights, the tall products of the deep-CCA backward) is a
-// chain of small and medium GEMMs.  Round 1 ran them as 64x64 FMA tiles on the CUDA cores; this kernel puts
-// them on the tensor pipe with the machinery K1 established:
+// chain of small and medium GEMMs.  This kernel puts them on the tensor pipe with the machinery of K1:
 //
-//   * operands straight from row-major storage by TMA, both majors: an operand whose reduction index is
-//     contiguous in memory lands K-major (32-float = 128-byte rows, SWIZZLE_128B), one whose reduction index is
-//     the strided one lands MN-major (32-column atoms, SWIZZLE_128B with 32-byte chunks -- the only legal
-//     MN-major TF32 layout, see moments.cu); the instruction descriptor carries one major bit per operand, so
-//     all four op() combinations of ccab_gemm map to the same mainloop without any transposed copy;
-//   * 3xTF32 with the split formed IN SHARED MEMORY: the tensor core truncates fp32 operands to TF32, so the raw
-//     tile is its own "hi" part; four converter warps derive lo = rna_tf32(x - trunc(x)) from the landed tile
-//     into a second buffer of the stage (generic-proxy stores, fence.proxy.async, mbarrier) while the MMA warp
-//     works on the previous stage -- no pre-pass over global memory, no second TMA stream;
-//   * fp32 accumulator in TMEM (128 lanes x BN columns), warp-specialised: warp 0 TMA producer, warp 1
-//     single-thread MMA issuer, warps 2-5 converters and, after the mainloop, the TMEM -> register -> global
-//     epilogue (alpha / beta, optional transposed copy, optional lower-triangle-only tiles);
-//   * batched through the third TMA coordinate (blockIdx.z).
+//   * operands straight from row-major storage, both majors: wgmma reads TF32 operands only K-major, so the
+//     256 threads of the CTA stage each 32-index slice of op(A) and op(B) into K-major 128-byte swizzled shared
+//     tiles (TileStager: float4 loads along a contiguous reduction index, a transposing store otherwise), and all
+//     four op() combinations of ccab_gemm share one mainloop without any transposed copy in global memory;
+//   * 3xTF32 with the split formed while staging: hi = truncated fp32, lo = rna_tf32(x - hi), three wgmmas per
+//     k-step (lo*hi, hi*lo, hi*hi); double-buffered, the global loads of the next slice in flight during the MMAs;
+//   * 128 x BN output tiles, two warpgroups of 64 rows each; the fp32 register accumulator of the tensor cores is
+//     added into a second register set after every slice (round-to-nearest adds), which keeps a K = 512 product at
+//     fp32 grade;
+//   * batched through blockIdx.z.
 //
-// Out-of-range rows / columns / reduction indices are zero-filled by TMA, so no shape needs padding.
+// Out-of-range rows / columns / reduction indices are staged as zeros, so no shape needs padding.
 // Replaces the FMA products behind cca_zoo/linear/_rcca.py:96,100, cca_zoo/linear/_mcca.py:131 and
 // cca_zoo/deep/objectives.py:97 (and the LAPACK level-3 calls inside scipy.linalg.eigh / numpy.linalg.svd).
 #include "tgemm.cuh"
 
-#include <mutex>
-
 namespace ccab {
 namespace {
 
-constexpr int kTgThreads = 192;
+constexpr int kTgThreads = 256;
 constexpr int kBM = 128;
-constexpr int kKC = 32;       // reduction indices per stage = one 128-byte swizzle row of a K-major tile
-constexpr int kAtom = kKC * 128;  // bytes of one 32-column MN-major atom
+constexpr int kKC = 32;       // reduction indices per slice = one 128-byte K-major row
+constexpr int kRun = 1;       // slices per accumulator run (32 reduction indices)
 
-struct alignas(64) TgParams {
-  CUtensorMap mapA, mapB;
+struct TgParams {
+  const float* A;
+  const float* B;
+  long long lda, strideA, strideA2, ldb, strideB, strideB2;
   float* C;
   long long ldc, strideC, strideC2;
   float* Ct;
@@ -49,250 +45,113 @@ struct alignas(64) TgParams {
 
 template <int BN>
 struct TgCfg {
-  static constexpr int kABytes = kBM * kKC * 4;
-  static constexpr int kBBytes = BN * kKC * 4;
-  static constexpr int kRaw = kABytes + kBBytes;
-  static constexpr int kStage = 2 * kRaw;  // raw (= hi) tiles, then the lo tiles at the same offsets
-  static constexpr int kStages = BN == 128 ? 3 : 4;
-  // tcgen05 accumulates with round-toward-zero: one accumulator drifts by ~0.5 ulp per MMA (1e-5 relative after
-  // 1024 reduction indices, measured).  The reduction is therefore dealt round-robin, one 32-index chunk at a time,
-  // over kSegs independent TMEM accumulators that the epilogue adds in registers (round-to-nearest).
-  static constexpr int kSegs = 512 / BN;
-  static constexpr int kSmem = kStages * kStage + 1024 + 256;
+  static constexpr int kATile = kBM * kKC * 4;
+  static constexpr int kBTile = BN * kKC * 4;
+  static constexpr int kStage = 2 * (kATile + kBTile);  // A hi, A lo, B hi, B lo
+  static constexpr int kSmem = 2 * kStage + 1024;
 };
 
 template <bool AK, bool BK, int BN>
 __global__ void __launch_bounds__(kTgThreads, 1) tgemm_kernel(const __grid_constant__ TgParams p) {
   using Cfg = TgCfg<BN>;
-  constexpr int NS = Cfg::kStages;
+  constexpr int R = BN / 2;   // accumulator registers per thread
   const int m0 = blockIdx.y * kBM, n0 = blockIdx.x * BN;
   const int bz = (int)blockIdx.z % p.batch1, bz2 = (int)blockIdx.z / p.batch1;
   if (p.lower_only && n0 >= m0 + kBM) return;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + NS * Cfg::kStage);
-  uint64_t* conv_bar = full_bar + NS;
-  uint64_t* empty_bar = conv_bar + NS;
-  uint64_t* tmem_full_bar = empty_bar + NS;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int nchunks = (p.K + kKC - 1) / kKC;
+  // op(A) row m, reduction index k: A[m * lda + k] (AK) or A[k * lda + m]; op(B)^T row n likewise with BK
+  const float* Ab = p.A + (size_t)bz * p.strideA + (size_t)bz2 * p.strideA2 + (AK ? (size_t)m0 * p.lda : (size_t)m0);
+  const float* Bb = p.B + (size_t)bz * p.strideB + (size_t)bz2 * p.strideB2 + (BK ? (size_t)n0 * p.ldb : (size_t)n0);
+  const int nch = (p.K + kKC - 1) / kKC;
+  TileStager<AK, kBM> sa;
+  TileStager<BK, BN> sb;
+  auto load = [&](int c) {
+    const int k0 = c * kKC, ks = min(kKC, p.K - k0);
+    sa.load(Ab + (AK ? (size_t)k0 : (size_t)k0 * p.lda), p.lda, p.M - m0, ks, true);
+    sb.load(Bb + (BK ? (size_t)k0 : (size_t)k0 * p.ldb), p.ldb, p.N - n0, ks, true);
+  };
+  auto store = [&](int buf) {
+    uint8_t* st = smem + buf * Cfg::kStage;
+    sa.template store<true>(st, st + Cfg::kATile);
+    sb.template store<true>(st + 2 * Cfg::kATile, st + 2 * Cfg::kATile + Cfg::kBTile);
+  };
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < NS; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&conv_bar[s], 128);
-      mbar_init(&empty_bar[s], 1);
-    }
-    mbar_init(tmem_full_bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.mapA);
-    tma_prefetch_desc(&p.mapB);
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
+  float acc[R], tot[R];
+#pragma unroll
+  for (int i = 0; i < R; ++i) acc[i] = tot[i] = 0.f;
+  const int wg = threadIdx.x >> 7;
+  load(0);
+  store(0);
+  fence_proxy_async_smem();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ================= TMA producer =================
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int c = 0; c < nchunks; ++c) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        mbar_arrive_expect_tx(&full_bar[stage], Cfg::kRaw);
-        uint8_t* sA = smem + stage * Cfg::kStage;
-        uint8_t* sB = sA + Cfg::kABytes;
-        const int k0 = c * kKC;
-        if (AK) {
-          tma_load_4d(sA, &p.mapA, &full_bar[stage], k0, m0, bz, bz2);
-        } else {
+  for (int c = 0; c < nch; ++c) {
+    const uint32_t st = smem_u32(smem + (c & 1) * Cfg::kStage);
+    const uint32_t a0 = st + wg * 64 * 128, b0 = st + 2 * Cfg::kATile;
+    wgmma_fence();
 #pragma unroll
-          for (int a = 0; a < kBM / 32; ++a) tma_load_4d(sA + a * kAtom, &p.mapA, &full_bar[stage], m0 + 32 * a, k0, bz, bz2);
-        }
-        if (BK) {
-          tma_load_4d(sB, &p.mapB, &full_bar[stage], k0, n0, bz, bz2);
-        } else {
+    for (int kk = 0; kk < kKC / 8; ++kk) {
+      const uint64_t a_hi = wgmma_desc_k128(a0 + 32 * kk), a_lo = wgmma_desc_k128(a0 + Cfg::kATile + 32 * kk);
+      const uint64_t b_hi = wgmma_desc_k128(b0 + 32 * kk), b_lo = wgmma_desc_k128(b0 + Cfg::kBTile + 32 * kk);
+      wgmma_tf32<BN>(acc, a_lo, b_hi);   // small cross terms first
+      wgmma_tf32<BN>(acc, a_hi, b_lo);
+      wgmma_tf32<BN>(acc, a_hi, b_hi);
+    }
+    wgmma_commit();
+    const bool more = c + 1 < nch;
+    if (more) load(c + 1);
+    wgmma_wait_all();
+    wgmma_fence_regs<R>(acc);
+    if (!more || (c + 1) % kRun == 0) {
 #pragma unroll
-          for (int a = 0; a < BN / 32; ++a) tma_load_4d(sB + a * kAtom, &p.mapB, &full_bar[stage], n0 + 32 * a, k0, bz, bz2);
-        }
-        if (++stage == NS) { stage = 0; phase ^= 1; }
+      for (int i = 0; i < R; ++i) {
+        tot[i] += acc[i];
+        acc[i] = 0.f;
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    const uint32_t idesc = umma_idesc_tf32(kBM, BN, AK, BK);
-    // K-major: 8-row groups 1024 B apart (SBO), 128-byte swizzle (layout 2); a k-step of 8 floats = +32 B.
-    // MN-major: 32-column atoms kAtom apart (LBO), 4-row groups 512 B apart (SBO), layout 1; a k-step = +1024 B.
-    const uint64_t dA0 = AK ? umma_smem_desc(smem_u32(smem), 16, 1024, 2) : umma_smem_desc(smem_u32(smem), kAtom, 512, 1);
-    const uint64_t dB0 = BK ? umma_smem_desc(smem_u32(smem) + Cfg::kABytes, 16, 1024, 2)
-                            : umma_smem_desc(smem_u32(smem) + Cfg::kABytes, kAtom, 512, 1);
-    constexpr uint64_t stepA = AK ? 2 : 64, stepB = BK ? 2 : 64;
-    constexpr uint64_t lo_off = (uint64_t)(Cfg::kRaw >> 4);
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int c = 0; c < nchunks; ++c) {
-      mbar_wait(&conv_bar[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t so = (uint64_t)((stage * Cfg::kStage) >> 4);
-        const uint32_t tacc = tmem_base + (uint32_t)((c % Cfg::kSegs) * BN);
-        uint32_t acc = c >= Cfg::kSegs ? 1u : 0u;
+    if (more) store((c + 1) & 1);   // that stage was last read by the wgmmas of slice c - 1, retired before the barrier
+    fence_proxy_async_smem();
+    __syncthreads();
+  }
+
+  // ---- epilogue: fragment element r of a thread is (row lane/4 + 8*((r/2)%2), column 8*(r/4) + 2*(lane%4) + r%2)
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  float* Cb = p.C ? p.C + (size_t)bz * p.strideC + (size_t)bz2 * p.strideC2 : nullptr;
+  float* Ctb = p.Ct ? p.Ct + (size_t)bz * p.strideCt + (size_t)bz2 * p.strideCt2 : nullptr;
 #pragma unroll
-        for (int kk = 0; kk < kKC / 8; ++kk) {
-          const uint64_t a_hi = dA0 + so + kk * stepA, b_hi = dB0 + so + kk * stepB;
-          umma_tf32(tacc, a_hi + lo_off, b_hi, idesc, acc);   // small cross terms first
-          umma_tf32(tacc, a_hi, b_hi + lo_off, idesc, 1u);
-          umma_tf32(tacc, a_hi, b_hi, idesc, 1u);
-          acc = 1u;
+  for (int r = 0; r < R; r += 2) {
+    const int row = m0 + wg * 64 + warp * 16 + (lane >> 2) + 8 * ((r >> 1) & 1);
+    const int col = n0 + 8 * (r >> 2) + 2 * (lane & 3);
+    if (row >= p.M) continue;
+    float v0 = p.alpha * tot[r], v1 = p.alpha * tot[r + 1];
+    if (Cb) {
+      float* crow = Cb + (size_t)row * p.ldc + col;
+      if (p.vec_c && col + 2 <= p.N) {   // col is even and ldc % 4 == 0: an aligned float2
+        float2* c2 = reinterpret_cast<float2*>(crow);
+        if (p.beta != 0.f) {
+          const float2 o = *c2;
+          v0 += p.beta * o.x;
+          v1 += p.beta * o.y;
         }
-        umma_commit(&empty_bar[stage]);
-      }
-      __syncwarp();
-      if (++stage == NS) { stage = 0; phase ^= 1; }
-    }
-    if (elect_one()) umma_commit(tmem_full_bar);
-    __syncwarp();
-  } else {
-    // ================= converters: lo = rna_tf32(x - trunc_tf32(x)) of the landed stage =================
-    const int tid = threadIdx.x - 64;
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int c = 0; c < nchunks; ++c) {
-        mbar_wait(&full_bar[stage], phase);
-        const float4* src = reinterpret_cast<const float4*>(smem + stage * Cfg::kStage);
-        float4* dst = reinterpret_cast<float4*>(smem + stage * Cfg::kStage + Cfg::kRaw);
-#pragma unroll 4
-        for (int i = tid; i < Cfg::kRaw / 16; i += 128) {
-          const float4 v = src[i];
-          dst[i] = make_float4(tf32_residual(v.x), tf32_residual(v.y), tf32_residual(v.z), tf32_residual(v.w));
+        *c2 = make_float2(v0, v1);
+      } else {
+        if (col < p.N) {
+          if (p.beta != 0.f) v0 += p.beta * crow[0];
+          crow[0] = v0;
         }
-        fence_proxy_async_smem();
-        mbar_arrive(&conv_bar[stage]);
-        if (++stage == NS) { stage = 0; phase ^= 1; }
+        if (col + 1 < p.N) {
+          if (p.beta != 0.f) v1 += p.beta * crow[1];
+          crow[1] = v1;
+        }
       }
     }
-    // ================= epilogue =================
-    const int g = warp & 3;
-    const int row = m0 + g * 32 + lane;
-    const int nsegs = nchunks < Cfg::kSegs ? nchunks : Cfg::kSegs;
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    float* Cb = p.C ? p.C + (size_t)bz * p.strideC + (size_t)bz2 * p.strideC2 : nullptr;
-    float* Ctb = p.Ct ? p.Ct + (size_t)bz * p.strideCt + (size_t)bz2 * p.strideCt2 : nullptr;
-#pragma unroll 1
-    for (int cc = 0; cc < BN / 32; ++cc) {
-      const int col0 = n0 + cc * 32;
-      if (col0 >= p.N) break;   // warp-uniform
-      float v[32];
-      {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(g * 32) << 16) + cc * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-      }
-      for (int sgm = 1; sgm < nsegs; ++sgm) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(g * 32) << 16) + sgm * BN + cc * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] += __uint_as_float(r[i]);
-      }
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] *= p.alpha;
-      if (Cb && row < p.M) {
-        float* crow = Cb + (size_t)row * p.ldc + col0;
-        if (p.vec_c && col0 + 32 <= p.N) {
-          float4* c4 = reinterpret_cast<float4*>(crow);
-          if (p.beta != 0.f) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const float4 o = c4[q];
-              v[4 * q] += p.beta * o.x; v[4 * q + 1] += p.beta * o.y; v[4 * q + 2] += p.beta * o.z; v[4 * q + 3] += p.beta * o.w;
-            }
-          }
-#pragma unroll
-          for (int q = 0; q < 8; ++q) c4[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            if (col0 + i < p.N) {
-              if (p.beta != 0.f) v[i] += p.beta * crow[i];
-              crow[i] = v[i];
-            }
-          }
-        }
-      } else if (!Cb && p.beta != 0.f) {
-        // unreachable: the host rejects beta != 0 without C
-      }
-      if (Ctb && row < p.M) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (col0 + i < p.N) Ctb[(size_t)(col0 + i) * p.ldct + row] = v[i];   // lanes = consecutive rows: coalesced
-      }
+    if (Ctb) {
+      if (col < p.N) Ctb[(size_t)col * p.ldct + row] = v0;
+      if (col + 1 < p.N) Ctb[(size_t)(col + 1) * p.ldct + row] = v1;
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(f);
-  });
-  return fn;
-}
-
-// K-major operand: stored (rows x K) row-major, box = 32 reduction indices x `box_rows` rows.
-// MN-major operand: stored (K x cols) row-major, box = 32 columns x 32 reduction indices.
-int encode_operand(CUtensorMap* map, const float* ptr, bool kmajor, int64_t mn, int64_t k, int64_t ld, int64_t stride,
-                   int batch, int64_t stride2, int batch2, int box_rows) {
-  EncodeTiledFn enc = encode_fn();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled entry point not available (driver too old?)");
-    return -2;
-  }
-  const int64_t outer = kmajor ? mn : k;
-  if (batch == 1) stride = ld * outer;     // unused dimension: any valid (16-byte multiple) stride
-  if (batch2 == 1) stride2 = ld * outer;
-  cuuint64_t gdim[4] = {(cuuint64_t)(kmajor ? k : mn), (cuuint64_t)outer, (cuuint64_t)batch, (cuuint64_t)batch2};
-  cuuint64_t gstride[3] = {(cuuint64_t)ld * 4, (cuuint64_t)stride * 4, (cuuint64_t)stride2 * 4};
-  cuuint32_t box[4] = {32, (cuuint32_t)(kmajor ? box_rows : kKC), 1, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   kmajor ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed with CUresult %d (mn=%lld k=%lld ld=%lld stride=%lld batch=%d)", (int)r,
-              (long long)mn, (long long)k, (long long)ld, (long long)stride, batch);
-    return -3;
-  }
-  return 0;
 }
 
 template <bool AK, bool BK, int BN>
@@ -325,14 +184,6 @@ bool tgemm_supported(const TgemmArgs& a) {
 }
 
 int tgemm(const TgemmArgs& a, cudaStream_t stream) {
-  {
-    // cuTensorMapEncodeTiled is a driver entry point and needs a current context on the CALLING thread; a thread that
-    // has only inherited the device ordinal (torch's autograd worker) has none until a runtime call binds the primary
-    // context -- cudaSetDevice does (CUDA 12)
-    int dev = 0;
-    CCAB_CUDA(cudaGetDevice(&dev));
-    CCAB_CUDA(cudaSetDevice(dev));
-  }
   CCAB_CHECK_ARG(tgemm_supported(a), "tgemm: operands must be 16-byte aligned with leading dimensions % 4 == 0");
   CCAB_CHECK_ARG(a.C || a.Ct, "tgemm: no output");
   CCAB_CHECK_ARG(a.C || a.beta == 0.f, "tgemm: beta != 0 needs C");
@@ -344,10 +195,14 @@ int tgemm(const TgemmArgs& a, cudaStream_t stream) {
   if (a.force_bn == 64 || a.force_bn == 128) BN = a.force_bn;
   TgParams prm;
   memset(&prm, 0, sizeof(prm));
-  int rc = encode_operand(&prm.mapA, a.A, AK, a.m, a.k, a.lda, a.strideA, a.batch, a.strideA2, a.batch2, kBM);
-  if (rc) return rc;
-  rc = encode_operand(&prm.mapB, a.B, BK, a.n, a.k, a.ldb, a.strideB, a.batch, a.strideB2, a.batch2, BN);
-  if (rc) return rc;
+  prm.A = a.A;
+  prm.lda = a.lda;
+  prm.strideA = a.strideA;
+  prm.strideA2 = a.strideA2;
+  prm.B = a.B;
+  prm.ldb = a.ldb;
+  prm.strideB = a.strideB;
+  prm.strideB2 = a.strideB2;
   prm.C = a.C;
   prm.ldc = a.ldc;
   prm.strideC = a.strideC;

@@ -1,4 +1,4 @@
-// Rectangular fp32 GEMM on the 5th-generation tensor cores (tcgen05.mma kind::tf32, 3xTF32 split formed in
+// Rectangular fp32 GEMM on the Hopper tensor cores (wgmma TF32, 3xTF32 split formed while staging into
 // shared memory) -- the solver-stage companion of the moment kernel K1.  See tgemm.cu.
 #pragma once
 #include "common.cuh"
@@ -24,7 +24,7 @@ struct TgemmArgs {
   int lower_only = 0;             // skip 128 x BN tiles that lie strictly above the diagonal (SYRK-type updates)
 };
 
-// TMA needs 16-byte aligned base pointers / leading dimensions / batch strides.  False -> use the FMA kernel.
+// The staging loads need 16-byte aligned base pointers / leading dimensions / batch strides.  False -> use the FMA kernel.
 bool tgemm_supported(const TgemmArgs& a);
 
 // Asynchronous on `stream`.  Returns 0, <0 bad argument, >0 cudaError_t.

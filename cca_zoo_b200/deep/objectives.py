@@ -26,7 +26,7 @@ from .. import ops
 
 def _require_cuda(name, *tensors):
     if not all(t.is_cuda for t in tensors):
-        raise RuntimeError(f"cca_zoo_b200.{name} needs CUDA tensors (sm_100a); there is no CPU fallback.")
+        raise RuntimeError(f"cca_zoo_b200.{name} needs CUDA tensors (sm_90a); there is no CPU fallback.")
 
 
 def _row_major(z):
@@ -35,7 +35,7 @@ def _row_major(z):
 
 
 def _resolve_precision(precision, zs):
-    """"auto": exact FMA moments for narrow batches (HBM / latency bound), the tcgen05 3xTF32 kernel once the block
+    """"auto": exact FMA moments for narrow batches (HBM / latency bound), the wgmma 3xTF32 kernel once the block
     covariance is wide enough to be a real contraction -- if TMA can address the representations."""
     if zs[0].dtype == torch.float64:
         return "exact"
@@ -159,7 +159,7 @@ class CCALoss(nn.Module):
     Args:
         eps: ridge added to the within-view covariances and eigenvalue floor (default 1e-5).
         precision: arithmetic of the covariance kernel for float32 inputs: ``"auto"`` (default: exact CUDA-core FMA
-            for narrow representations, tcgen05 3xTF32 beyond a total width of 256), ``"exact"``, ``"tf32x3"``, ``"tf32"``.
+            for narrow representations, wgmma 3xTF32 beyond a total width of 256), ``"exact"``, ``"tf32x3"``, ``"tf32"``.
         verify: ``"lazy"`` (default) never reads anything back in ``forward``: the Cholesky status of every
             evaluation is copied to the host asynchronously and inspected at the next call / by ``check()``, which
             raise if an earlier batch had a numerically indefinite covariance.  ``"sync"`` reads the status back in

@@ -23,7 +23,7 @@ class rCCA(BaseModel):
     Same estimator as ``cca_zoo.linear.rCCA`` (cca_zoo/linear/_rcca.py:16-101): maximise
     :math:`w_1^\top X_1^\top X_2 w_2` s.t. :math:`w_i^\top((1-c_i) X_i^\top X_i + c_i I) w_i = 1`.
     The reference whitens each view with a tall SVD and takes the SVD of the whitened
-    cross-covariance; here the same weights come from the block covariance (one tcgen05 pass over
+    cross-covariance; here the same weights come from the block covariance (one tensor-core pass over
     the data) and small Jacobi eigen/singular-value solves on the device.
 
     Args:

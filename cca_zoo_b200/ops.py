@@ -17,7 +17,7 @@ _DT = {torch.float32: _lib.F32, torch.float64: _lib.F64}
 def _require_cuda(t: torch.Tensor, name: str) -> None:
     if not t.is_cuda:
         raise RuntimeError(
-            f"{name} must be a CUDA tensor: cca_zoo_b200 runs on sm_100a only and has no CPU fallback"
+            f"{name} must be a CUDA tensor: cca_zoo_b200 runs on sm_90a only and has no CPU fallback"
         )
 
 

@@ -1,4 +1,4 @@
-/* libccab200 -- C ABI of the B200-native CCA hot path.
+/* libccab200 -- C ABI of the H100-native CCA hot path.
  *
  * The reference (jameschapman19/cca_zoo) is pure Python and has NO FFI boundary for this path
  * (SURVEY.md §8b); this header is the boundary a maintainer would bind with ctypes (see
@@ -13,7 +13,7 @@
  *     ccab_gesvj which synchronise it once per Jacobi sweep to read the convergence flag;
  *   - return 0 = OK, <0 = bad argument / unsupported, >0 = cudaError_t.  ccab_last_error() gives the
  *     message of the last failure on the calling thread.  No C++ exception crosses the ABI.
- *   - dtype: CCAB_F32 / CCAB_F64.  There is no CPU fallback: without a sm_100a device every compute
+ *   - dtype: CCAB_F32 / CCAB_F64.  There is no CPU fallback: without a sm_90a device every compute
  *     entry point fails.
  */
 #ifndef CCAB200_H
@@ -30,8 +30,8 @@ extern "C" {
 #define CCAB_F64 1
 
 /* arithmetic of the moment kernel (ccab_moments `precision`) */
-#define CCAB_PREC_TF32 0   /* fp32 in, one tcgen05 kind::tf32 pass, fp32 accumulate               */
-#define CCAB_PREC_TF32X3 1 /* fp32 in, hi/lo split + 3 tcgen05 passes: fp32-grade accuracy          */
+#define CCAB_PREC_TF32 0   /* fp32 in, one wgmma TF32 pass, fp32 accumulate               */
+#define CCAB_PREC_TF32X3 1 /* fp32 in, hi/lo split + 3 wgmma passes: fp32-grade accuracy          */
 #define CCAB_PREC_EXACT 2  /* FMA in the input dtype on CUDA cores (the only choice for CCAB_F64)  */
 #define CCAB_PREC_TF32X3B 3 /* 3xTF32 with the two cross terms as bf16 MMAs (kind::f16): fp32-grade, 2/3 the tensor work */
 
@@ -158,7 +158,7 @@ int ccab_gesvj(int dtype, int m, int n, const void* A, int64_t lda, void* sigma,
 int ccab_gemm(int dtype, int transa, int transb, int m, int n, int k, double alpha, const void* A, int64_t lda,
               const void* B, int64_t ldb, double beta, void* C, int64_t ldc, void* stream);
 
-/* Tensor-core variant of ccab_gemm for float32 (tcgen05.mma kind::tf32, 3xTF32 split formed in shared memory:
+/* Tensor-core variant of ccab_gemm for float32 (wgmma TF32, 3xTF32 split formed in shared memory:
  * fp32-grade products, fp32 accumulation in TMEM), batched: matrix b of the batch lives at X + b * stride_x.
  * Optionally also (or only: C may be NULL when beta == 0) writes the transpose Ct (n x m, row-major, ldct).
  * lower_only != 0 skips the 128-row output tiles that lie strictly above the diagonal (SYRK-type updates).
@@ -212,7 +212,7 @@ int ccab_trsm(int dtype, int side, int trans, int n, int m, const void* L, int64
  * info_dev[b] (device int[batch]) = 0 or the 1-based index of the first pivot <= pivot_tol.
  * Diagonal blocks (128 wide for float, 64 for double) are factored AND inverted by one single-CTA launch each
  * (warp-synchronous 32 x 32 sub-blocks); panels, trailing updates and the assembly of L^-1 by recursive doubling are
- * GEMMs (tcgen05 for float).  With Linv,  T = L1^-1 C12 L2^-T  and the weights  L_i^-T U_k  are plain products.
+ * GEMMs (wgmma for float).  With Linv,  T = L1^-1 C12 L2^-T  and the weights  L_i^-T U_k  are plain products.
  * Replaces LAPACK potrf / trsm inside scipy.linalg.eigh(A, B) (cca_zoo/_utils/_linalg.py:67-71) and, in Cholesky
  * form, the whitening of cca_zoo/_utils/_linalg.py:30-38 and _inv_sqrtm of cca_zoo/deep/objectives.py:9-21. */
 size_t ccab_potrf_inv_workspace_bytes(int dtype, int n, int batch);
@@ -232,7 +232,7 @@ int ccab_potrf_inv(int dtype, int n, int batch, void* A, int64_t lda, int64_t st
  *                 8 too few samples (n <= max d_i);  header[1] = n_total;  [2] residual;  [3] sigma_1;
  *                 [4] index of the first failed factorisation;  [5] sweeps of the Ritz eigensolve
  *   n_total_dev (device double, may be NULL) overrides n_total: the sample count can ride in the all-reduced message.
- *   p must satisfy k <= p <= min(d1, d2, 128).  dtype = arithmetic of the whole solve (CCAB_F32 uses tcgen05 GEMMs).
+ *   p must satisfy k <= p <= min(d1, d2, 128).  dtype = arithmetic of the whole solve (CCAB_F32 uses wgmma GEMMs).
  * Replaces cca_zoo/linear/_rcca.py:83-101 (via cca_zoo/_utils/_linalg.py:9-41) after the moment pass. */
 size_t ccab_rcca_fit_workspace_bytes(int dtype, const int64_t* dims, int k, int p);
 int ccab_rcca_fit_result_layout(int dtype, const int64_t* dims, int k, int p, int64_t* offsets /* [5] */);
@@ -264,7 +264,7 @@ int ccab_mcca_fit(int dtype, int n_views, const int64_t* dims, const double* mom
  * rounding destroyed the ridge; the caller re-runs through the eigen route, which clamps like the reference) and a
  * non-finite-input flag -- check lazily.
  * ccab_ccaloss_bwd: g1 = 2/(n-1) center(z1 G11 - z2 P^T) * grad_out[0], g2 = 2/(n-1) center(z2 G22 - z1 P) * grad_out[0]
- * (grad_out: device scalar, may be NULL = 1).  4 tall GEMMs (tcgen05 for float) + the centring (slab partial sums in a
+ * (grad_out: device scalar, may be NULL = 1).  4 tall GEMMs (wgmma for float) + the centring (slab partial sums in a
  * 2 MB per-device scratch that this entry point allocates on first use -- the one exception to "the library never
  * allocates": it takes no workspace argument); widths <= 64 run as ONE fused launch instead.
  * Replaces cca_zoo/deep/objectives.py:9-21,79-102 and torch autograd through two eigh + eigvalsh. */
@@ -288,7 +288,7 @@ int ccab_center_columns(int dtype, int m, int n, void* A, int64_t lda, void* str
 int ccab_frobenius_norm(int dtype, int m, int n, const void* A, int64_t lda, void* out, void* stream);
 
 /* Measurement hook: when enabled, CUDA events are recorded on the caller's stream immediately around the
- * tcgen05 moment-kernel launch of ccab_moments (TF32 paths); ccab_profile_moments_last_ms() waits for the
+ * tensor-core moment-kernel launch of ccab_moments (TF32 paths); ccab_profile_moments_last_ms() waits for the
  * last pair and returns the kernel's duration in ms (-1 if none). */
 int ccab_profile_moments(int enable);
 double ccab_profile_moments_last_ms(void);

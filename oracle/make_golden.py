@@ -139,6 +139,10 @@ def main():
 
     gdir = os.path.join(ROOT, "tests", "golden")
     os.makedirs(gdir, exist_ok=True)
+    # the large float64 arrays keep 30 of their 52 mantissa bits (relative rounding <= 1e-9, far below every tolerance
+    # they are checked with), which keeps the compressed file under 1 MB
+    out = {k: (v.view(np.uint64) & ~np.uint64((1 << 22) - 1)).view(np.float64)
+           if v.dtype == np.float64 and v.nbytes >= 16384 else v for k, v in out.items()}
     np.savez_compressed(os.path.join(gdir, "reference_outputs.npz"), **out)
     with open(os.path.join(gdir, "reference_outputs.json"), "w") as f:
         json.dump(meta, f, indent=1)

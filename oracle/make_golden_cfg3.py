@@ -75,6 +75,10 @@ def main():
         meta["cases"].append(dict(name=name, kind=kind, batch=batch, widths=widths, eps=eps, seed=seed))
         print(name, loss.item())
     gdir = os.path.join(ROOT, "tests", "golden")
+    # the large float64 arrays keep 30 of their 52 mantissa bits (relative rounding <= 1e-9, far below every tolerance
+    # they are checked with), which keeps the compressed file under 1 MB
+    out = {k: (v.view(np.uint64) & ~np.uint64((1 << 22) - 1)).view(np.float64)
+           if v.dtype == np.float64 and v.nbytes >= 16384 else v for k, v in out.items()}
     np.savez_compressed(os.path.join(gdir, "reference_outputs_cfg3.npz"), **out)
     with open(os.path.join(gdir, "reference_outputs_cfg3.json"), "w") as f:
         json.dump(meta, f, indent=1)

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (ccab_gemm_tc) against a float64 torch product: every op() combination (= every pairing of
+"""wgmma GEMM (ccab_gemm_tc) against a float64 torch product: every op() combination (= every pairing of
 K-major / MN-major shared-memory operands), ragged sizes (TMA zero fill), batches, alpha / beta, the transposed
 copy and the lower-triangle-only mode.  Tolerance: fp32-grade (3xTF32 products, fp32 accumulation)."""
 import pytest

@@ -1,10 +1,11 @@
-"""Differential fuzzing of the HOST-SIDE logic against the live reference (authoring container only: needs
-/root/reference): random shapes, ridge values, centring flags, view weights, confounds, feature groups, dtypes.
+"""Differential fuzzing of the HOST-SIDE logic against the reference: random shapes, ridge values, centring flags, view weights, confounds, feature groups, dtypes.
 The kernels are replaced by tests/fake_ops.py (torch CPU), so every mismatch is a divergence of the Python between
 the kernels from the reference's behaviour.  Ill-posed draws (c = 0 with a rank-deficient or under-determined view,
 where the reference itself returns noise-dependent output) are reported only with --all.
+With --golden the reference's results come from tests/golden/reference_fuzz.npz (recorded for seed 20240924,
+200 trials by oracle/make_golden_live.py), so no reference installation is needed.
 
-    python tools/fuzz_vs_reference.py [seed] [trials] [--all]
+    python tools/fuzz_vs_reference.py [seed] [trials] [--all] [--medium] [--golden]
 """
 import os
 import sys
@@ -17,23 +18,14 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from tests import fake_ops  # noqa: E402  (before refshim: the reference has its own `tests` package)
 from oracle import refshim  # noqa: E402
-
-refshim.install()
-import cca_zoo.linear as ref  # noqa: E402
-
-fake_ops.install(pytest.MonkeyPatch())
-from cca_zoo_b200 import linear as ours  # noqa: E402
 from oracle import restatement as R  # noqa: E402
 
+GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_fuzz.npz")
 
-def main():
-    args = [a for a in sys.argv[1:] if not a.startswith("--")]
-    seed = int(args[0]) if args else 0
-    trials = int(args[1]) if len(args) > 1 else 300
-    show_all = "--all" in sys.argv
-    medium = "--medium" in sys.argv        # wider views, explicit solver routes (top-k route needs 4k <= width)
+
+def draw_trials(seed, trials, medium=False):
+    """The seeded problems, independent of any result: (model, views, kw, ours_kw, extra, facts)."""
     rng = np.random.default_rng(seed)
-    bad = 0
     for _ in range(trials):
         model = str(rng.choice(["CCA", "rCCA", "PLS", "MCCA", "GCCA", "PartialCCA", "GRCCA"]))
         m = 2 if model in ("CCA", "rCCA", "PLS") else int(rng.integers(2, 5))
@@ -79,59 +71,123 @@ def main():
         # c = 0 needs full-rank blocks; GCCA takes pinv(view) whatever c is; float32 inputs of an under-determined
         # problem amplify the reference's own float32 rounding (centring and pinv run in float32 there)
         well = determined or (cmin > 0 and model != "GCCA" and not f32)
-        desc = f"{'well ' if well else 'ILL  '}{model} n={n} dims={dims} f32={f32} {kw} {ours_kw}"
-        out = []
-        for lib in (ref, ours):
-            try:
-                with warnings.catch_warnings():
-                    warnings.simplefilter("ignore")
-                    est = getattr(lib, model)(**kw, **(ours_kw if lib is ours else {})).fit(views, **extra)
-                    held = [v[: n // 2] for v in views]
-                    out.append((est, est.score(views), est.transform(held), est.pairwise_correlations(held)))
-            except Exception as e:  # noqa: BLE001
-                out.append(e)
-        r, o = out
-        if isinstance(r, Exception) or isinstance(o, Exception):
-            if type(r) is not type(o):
-                bad += 1
-                print("EXCEPTION", desc, "| ref:", repr(r)[:120], "| ours:", repr(o)[:120])
-            continue
-        if not well and not show_all:
-            continue
-        if [w.shape for w in r[0].weights_] != [w.shape for w in o[0].weights_]:
+        facts = dict(n=n, dims=dims, q=q, f32=f32, well=well,
+                     desc=f"{'well ' if well else 'ILL  '}{model} n={n} dims={dims} f32={f32} {kw} {ours_kw}")
+        yield model, views, kw, ours_kw, extra, facts
+
+
+def run(lib, model, views, kw, extra):
+    """What a caller sees: (weights_, means_, score, transform of the held-out half, pairwise correlations), or the
+    name of the exception the fit raised."""
+    try:
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            est = getattr(lib, model)(**kw).fit(views, **extra)
+            held = [v[: views[0].shape[0] // 2] for v in views]
+            return dict(weights=list(est.weights_), means=[np.asarray(m) for m in est.means_],
+                        score=np.asarray(est.score(views)), transform=[np.asarray(t) for t in est.transform(held)],
+                        pairwise=np.asarray(est.pairwise_correlations(held)))
+    except Exception as e:  # noqa: BLE001
+        return type(e).__name__
+
+
+def to_arrays(i, res, out):
+    """Flatten one reference result into npz entries under trial index i."""
+    if isinstance(res, str):
+        out[f"{i}/exception"] = np.array(res)
+        return
+    for key in ("weights", "means", "transform"):
+        for j, a in enumerate(res[key]):
+            out[f"{i}/{key}{j}"] = a
+    out[f"{i}/score"], out[f"{i}/pairwise"] = res["score"], res["pairwise"]
+
+
+def from_arrays(i, npz):
+    if f"{i}/exception" in npz:
+        return str(npz[f"{i}/exception"])
+    if f"{i}/score" not in npz:
+        return None    # ill-posed trial that did not raise: only its exception behaviour is compared
+    res = {"score": npz[f"{i}/score"], "pairwise": npz[f"{i}/pairwise"]}
+    for key in ("weights", "means", "transform"):
+        res[key], j = [], 0
+        while f"{i}/{key}{j}" in npz:
+            res[key].append(npz[f"{i}/{key}{j}"])
+            j += 1
+    return res
+
+
+def compare(r, o, facts, show_all=False):
+    """None if ours matches the reference's result r, else a description of the mismatch."""
+    desc = facts["desc"]
+    if isinstance(r, str) or isinstance(o, str):
+        return None if r == o else f"EXCEPTION {desc} | ref: {r} | ours: {o if isinstance(o, str) else 'no exception'}"
+    if r is None or (not facts["well"] and not show_all):
+        return None
+    if [w.shape for w in r["weights"]] != [w.shape for w in o["weights"]]:
+        return f"WEIGHT SHAPES {desc} {[w.shape for w in r['weights']]} {[w.shape for w in o['weights']]}"
+    dt_r = [w.dtype for w in r["weights"]] + [t.dtype for t in r["transform"]]
+    dt_o = [w.dtype for w in o["weights"]] + [t.dtype for t in o["transform"]]
+    if dt_r != dt_o:
+        return f"DTYPES {desc} {dt_r} {dt_o}"
+    tol = 2e-3 if facts["f32"] else 1e-6
+    kmax = min(min(facts["dims"]), max(facts["n"] - 2 - facts["q"], 0))
+    d_score = float(np.max(np.abs(r["score"] - o["score"])[np.arange(r["score"].shape[0]) < max(kmax, 1)]))
+    # weights / variates only for components that are determined: inside the rank of the problem, clearly
+    # correlated, and separated from both neighbours (sign-aligned per component)
+    sc = r["score"]
+    left = np.abs(np.diff(np.concatenate([[2.0], sc])))
+    right = np.abs(np.diff(np.concatenate([sc, [-2.0]])))
+    simple = (left > 1e-3) & (right > 1e-3) & (np.abs(sc) > 1e-3) & (np.arange(sc.shape[0]) < kmax)
+    w_r = [np.asarray(w, dtype=np.float64) for w in r["weights"]]
+    w_o = R.align_signs([np.asarray(w, dtype=np.float64) for w in o["weights"]], w_r)
+    d_w = 0.0
+    for a, b in zip(w_o, w_r):
+        num = np.linalg.norm(a - b, axis=0)[simple]
+        den = np.linalg.norm(b, axis=0)[simple]
+        if num.size:
+            d_w = max(d_w, float(np.max(num / np.maximum(den, 1e-300))))
+    d_means = max(float(np.max(np.abs(np.asarray(a, dtype=np.float64) - np.asarray(b, dtype=np.float64))))
+                  for a, b in zip(r["means"], o["means"]))
+    d_pair = float(np.max(np.abs(r["pairwise"][..., simple] - o["pairwise"][..., simple]))) if simple.any() else 0.0
+    if not (d_score < tol and d_w < 50 * tol and d_means < 1e-5 and d_pair < 50 * tol):
+        return f"VALUES score {d_score:.1e} weights {d_w:.1e} means {d_means:.1e} pairwise {d_pair:.1e} {desc}"
+    return None
+
+
+def record(seed, trials):
+    """The reference's results for the seeded problems (well-posed trials in full, the others by exception only)."""
+    refshim.install()
+    import cca_zoo.linear as ref
+
+    out = {}
+    for i, (model, views, kw, _, extra, facts) in enumerate(draw_trials(seed, trials)):
+        res = run(ref, model, views, kw, extra)
+        if isinstance(res, str) or facts["well"]:
+            to_arrays(i, res, out)
+    return out
+
+
+def main():
+    args = [a for a in sys.argv[1:] if not a.startswith("--")]
+    seed = int(args[0]) if args else 0
+    trials = int(args[1]) if len(args) > 1 else 300
+    show_all = "--all" in sys.argv
+    medium = "--medium" in sys.argv        # wider views, explicit solver routes (top-k route needs 4k <= width)
+    golden = np.load(GOLDEN) if "--golden" in sys.argv else None
+    if golden is None:
+        refshim.install()
+        import cca_zoo.linear as ref
+    fake_ops.install(pytest.MonkeyPatch())
+    from cca_zoo_b200 import linear as ours
+
+    bad = 0
+    for i, (model, views, kw, ours_kw, extra, facts) in enumerate(draw_trials(seed, trials, medium)):
+        r = from_arrays(i, golden) if golden is not None else run(ref, model, views, kw, extra)
+        o = run(ours, model, views, {**kw, **ours_kw}, extra)
+        msg = compare(r, o, facts, show_all)
+        if msg:
             bad += 1
-            print("WEIGHT SHAPES", desc, [w.shape for w in r[0].weights_], [w.shape for w in o[0].weights_])
-            continue
-        dt_r = [w.dtype for w in r[0].weights_] + [np.asarray(t).dtype for t in r[2]]
-        dt_o = [w.dtype for w in o[0].weights_] + [np.asarray(t).dtype for t in o[2]]
-        if dt_r != dt_o:
-            bad += 1
-            print("DTYPES", desc, dt_r, dt_o)
-            continue
-        tol = 2e-3 if f32 else 1e-6
-        kmax = min(min(dims), max(n - 2 - q, 0))
-        d_score = float(np.max(np.abs(r[1] - o[1])[np.arange(r[1].shape[0]) < max(kmax, 1)])) if True else 0.0
-        # weights / variates only for components that are determined: inside the rank of the problem, clearly
-        # correlated, and separated from both neighbours (sign-aligned per component)
-        sc = r[1]
-        kmax = min(min(dims), max(n - 2 - q, 0))
-        left = np.abs(np.diff(np.concatenate([[2.0], sc])))
-        right = np.abs(np.diff(np.concatenate([sc, [-2.0]])))
-        simple = (left > 1e-3) & (right > 1e-3) & (np.abs(sc) > 1e-3) & (np.arange(sc.shape[0]) < kmax)
-        w_r = [np.asarray(w, dtype=np.float64) for w in r[0].weights_]
-        w_o = R.align_signs([np.asarray(w, dtype=np.float64) for w in o[0].weights_], w_r)
-        d_w = 0.0
-        for a, b in zip(w_o, w_r):
-            num = np.linalg.norm(a - b, axis=0)[simple]
-            den = np.linalg.norm(b, axis=0)[simple]
-            if num.size:
-                d_w = max(d_w, float(np.max(num / np.maximum(den, 1e-300))))
-        d_means = max(float(np.max(np.abs(np.asarray(a, dtype=np.float64) - np.asarray(b, dtype=np.float64))))
-                      for a, b in zip(r[0].means_, o[0].means_))
-        d_pair = float(np.max(np.abs(r[3][..., simple] - o[3][..., simple]))) if simple.any() else 0.0
-        if not (d_score < tol and d_w < 50 * tol and d_means < 1e-5 and d_pair < 50 * tol):
-            bad += 1
-            print(f"VALUES score {d_score:.1e} weights {d_w:.1e} means {d_means:.1e} pairwise {d_pair:.1e}", desc)
+            print(msg)
     print(f"seed {seed}: {trials} trials, {bad} mismatches")
     return 1 if bad else 0
 
