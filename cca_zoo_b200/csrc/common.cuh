@@ -1,6 +1,6 @@
 // Shared device/host helpers for libccab200 (sm_90a, Hopper).
 //
-// PTX wrappers for the warpgroup MMA (wgmma) and the shared-memory staging of its operands.
+// PTX wrappers for the warpgroup MMA (wgmma), mbarrier, TMA and the shared-memory staging of wgmma operands.
 // Everything is hand-written inline PTX; no CUTLASS/CuTe dependency.
 #pragma once
 
@@ -46,6 +46,60 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
+// Register budget of the calling warpgroup (all its threads execute it): producer warps hand registers back, MMA
+// warps take them.  N is a multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// ---------------------------------------------------------------------------------------------
+// mbarrier (shared-memory barrier with phase parity and a transaction count for TMA)
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void fence_mbar_init() {
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
+               : "memory");
+}
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
+  uint32_t ok;
+  asm volatile(
+      "{\n\t.reg .pred P1;\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
+      "selp.b32 %0, 1, 0, P1;\n\t}\n"
+      : "=r"(ok)
+      : "r"(smem_u32(bar)), "r"(parity)
+      : "memory");
+  return ok != 0;
+}
+// Waits for the phase of the given parity to complete.  Bounded: a protocol error traps (a CUDA error on the host)
+// instead of hanging the device.  No printf here: a call inside a wgmma pipeline makes ptxas serialise the wgmmas.
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > (1u << 25)) __trap();
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// TMA: 2-D tile load global -> shared, completion counted in bytes on an mbarrier.  Elements outside the tensor map's
+// extent arrive as zeros.  c0 is the contiguous (column) coordinate, c1 the row.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // Hopper warpgroup MMA (wgmma, sm_90a): four warps issue one asynchronous MMA whose operands are read from shared
@@ -57,6 +111,8 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// retires all but the most recently committed group
+__device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 // keeps the compiler from moving reads of the accumulators above the wait that retires the MMAs writing them
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(float* d) {

@@ -1,9 +1,10 @@
 // K1: block moments M = X^T X (+ column sums) of the hstacked views, upper block triangle only.
 //
 //   * moments_wgmma_kernel : Hopper wgmma (TF32, fp32 accumulators in registers), 128 x 128 tiles of the upper
-//     block triangle, split over the sample axis.  The sample slices are transposed into K-major swizzled shared
-//     tiles by the staging stores.  Optional 3xTF32 (hi / lo copies staged in shared memory, 3 MMAs per k-step) for
-//     fp32-grade accuracy.  Column sums are exact fp32 sums of the staged values.
+//     block triangle, split over the sample axis.  A producer / consumer pipeline on mbarriers: TMA loads of the raw
+//     sample slices, two transpose warpgroups that write them as K-major swizzled shared tiles, two wgmma
+//     warpgroups.  Optional 3xTF32 (hi / lo copies in shared memory, 3 MMAs per k-step) for fp32-grade accuracy.
+//     Column sums are exact fp32 sums of the loaded values.
 //   * moments_simt_kernel : exact FMA (fp32) tile kernel, the non-tensor reference path;
 //     moments_dmma_kernel : float64 inputs on the fp64 tensor pipe (mma.sync m8n8k4.f64).
 //   * reduce / covariance kernels (K2): fixed-order sum of the split partials into a double
@@ -72,42 +73,63 @@ TcDebug& tc_debug() {
 // =============================================================================================
 // wgmma kernel
 // =============================================================================================
-// One CTA = one 128 x 128 tile (A block bi, B block bj >= bi) of M over one split of the sample axis.  Its 256 threads
-// stage each 32-sample slice of both column blocks into K-major swizzled shared tiles (the sample index is the
-// strided one of row-major X, so the transpose is done by the staging stores), double-buffered: the global loads of
-// slice c + 1 are in flight while the two warpgroups run the wgmmas of slice c, each on 64 rows of the tile.
-// The 3xTF32 mode stages hi and lo copies and issues lo*hi + hi*lo + hi*hi per k-step.  Column sums are exact fp32
-// sums of the staged values, taken by the diagonal tiles.
+// One CTA = one 128 x 128 tile (A block bi, B block bj >= bi) of M over one split of the sample axis, taken in 32-sample
+// slices by four warpgroups that meet only on mbarriers:
+//   * thread 0 issues the TMA loads of the raw row-major [32 samples x 128 columns] box of each column block into a
+//     ring of raw stages (a diagonal tile loads only A).  Rows past n_rows and columns past the view's width arrive
+//     as zeros;
+//   * warpgroups 0 and 1 transpose each raw stage into the K-major, 128-byte-swizzled operand tiles wgmma reads (the
+//     sample index is the strided one of row-major X, and wgmma reads TF32 only K-major): hi, and in 3xTF32 mode lo,
+//     in a ring of operand stages.  Thread (h, m) owns column m and the 4-sample groups of parity h.  Diagonal tiles
+//     also take the exact fp32 column sums here;
+//   * warpgroups 2 and 3 each run the wgmmas of 64 rows of the tile, one slice of MMAs in flight while the next slice
+//     is transposed.  The 3xTF32 mode issues lo*hi + hi*lo + hi*hi per k-step.
+// The mainloop is bound by shared-memory traffic, about 272 KB per 3xTF32 slice of an off-diagonal tile: 32 KB of TMA
+// writes, 32 KB of transpose reads, 64 KB of hi / lo stores and 144 KB of wgmma operand reads.  A second transpose
+// warpgroup hides the latency of the transpose; deeper rings do not help.
 struct WgParams {
-  const float* view_ptr[kMaxViews];
-  int64_t view_ld[kMaxViews];
-  int view_dim[kMaxViews];
+  CUtensorMap map[kMaxViews];   // view v: {width, rows} fp32, row pitch lds[v], box 128 columns x 32 rows
   uint8_t blk_view[kMaxBlocks];
   int blk_col0[kMaxBlocks];
   float* partial;      // [S][Dp][Dp]
   float* partial_sum;  // [S][Dp]
   int64_t n_rows, rows_per_split;
+  int64_t row_base;    // first row of this pass in the tensor maps
   int nblocks, Dp;
 };
 static_assert(sizeof(WgParams) <= 4096, "kernel parameter space");
 
-constexpr int kWgThreads = 256;
+constexpr int kWgXpose = 256;              // two transpose warpgroups
+constexpr int kWgThreads = kWgXpose + 256;  // + two MMA warpgroups
 constexpr int kWgKC = 32;                  // samples per slice = one 128-byte K-major row
-constexpr int kWgTile = kBlk * kWgKC * 4;  // bytes of one staged 128 x 32 operand copy
+constexpr int kWgTile = kBlk * kWgKC * 4;  // bytes of one 128 x 32 fp32 tile (raw box or operand copy)
 
 template <bool X3>
 struct WgCfg {
-  static constexpr int kOps = X3 ? 2 : 1;           // hi (+ lo) copy of each operand
-  static constexpr int kStage = 2 * kOps * kWgTile;  // A copies, then B copies
-  static constexpr int kSmem = 2 * kStage + 1024;    // two stages + alignment slack
+  static constexpr int kOps = X3 ? 2 : 1;              // hi (+ lo) copy of each operand
+  static constexpr int kOpStage = 2 * kOps * kWgTile;  // A copies, then B copies
+  static constexpr int kRawStage = 2 * kWgTile;        // raw A box, raw B box
+  static constexpr int kOpStages = X3 ? 2 : 3;
+  static constexpr int kRawStages = X3 ? 3 : 4;
+  static constexpr int kBarOff = kOpStages * kOpStage + kRawStages * kRawStage;
+  static constexpr int kSumOff = kBarOff + 2 * (kOpStages + kRawStages) * 8;       // odd column sums
+  static constexpr int kSmem = kSumOff + kBlk * 4 + 1024;   // + alignment slack
 };
+static_assert(WgCfg<true>::kSmem <= 227 * 1024 && WgCfg<false>::kSmem <= 227 * 1024, "shared memory per block");
 
 template <bool X3>
 __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __grid_constant__ WgParams p) {
   using Cfg = WgCfg<X3>;
+  constexpr int NO = Cfg::kOpStages, NR = Cfg::kRawStages;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ float colsum_hi[kBlk];
+  // offset (not an integer round trip) so that the compiler still sees shared-memory pointers: LDS / STS, not LD / ST
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* ops = smem;                          // operand stages (1024-byte aligned: swizzle atoms)
+  uint8_t* raw = smem + NO * Cfg::kOpStage;     // raw stages
+  uint64_t* raw_full = reinterpret_cast<uint64_t*>(smem + Cfg::kBarOff);
+  uint64_t* raw_empty = raw_full + NR;
+  uint64_t* op_full = raw_empty + NR;
+  uint64_t* op_empty = op_full + NO;
 
   int t = blockIdx.x, bi = 0, rowlen = p.nblocks;   // tile decode over the upper block triangle
   while (t >= rowlen) { t -= rowlen; ++bi; --rowlen; }
@@ -118,80 +140,116 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
   const int64_t r1 = min(r0 + p.rows_per_split, p.n_rows);
   const int nch = r1 > r0 ? (int)((r1 - r0 + kWgKC - 1) / kWgKC) : 0;
 
-  const int vA = p.blk_view[bi], vB = p.blk_view[bj];
-  const float* XA = p.view_ptr[vA] + p.blk_col0[bi];
-  const float* XB = p.view_ptr[vB] + p.blk_col0[bj];
-  const int64_t ldA = p.view_ld[vA], ldB = p.view_ld[vB];
-  const int colsA = p.view_dim[vA] - p.blk_col0[bi], colsB = p.view_dim[vB] - p.blk_col0[bj];
-
-  TileStager<false, kBlk> sa, sb;
-  float csum = 0.f;   // column threadIdx.x % 128 of a diagonal tile, this thread's reduction indices
-  auto load = [&](int c) {
-    const int64_t r = r0 + (int64_t)c * kWgKC;
-    const int ks = (int)(r1 - r < kWgKC ? r1 - r : kWgKC);
-    sa.load(XA + r * ldA, ldA, colsA, ks, false);
-    if (!diag) sb.load(XB + r * ldB, ldB, colsB, ks, false);
-  };
-  auto store = [&](int buf) {
-    uint8_t* st = smem + buf * Cfg::kStage;
-    sa.template store<X3>(st, st + kWgTile);
-    if (!diag) sb.template store<X3>(st + Cfg::kOps * kWgTile, st + (Cfg::kOps + 1) * kWgTile);
-    if (diag) {
-#pragma unroll
-      for (int j = 0; j < TileStager<false, kBlk>::kItems; ++j) csum += (sa.v[j][0] + sa.v[j][1]) + (sa.v[j][2] + sa.v[j][3]);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NR; ++s) {
+      mbar_init(&raw_full[s], 1);
+      mbar_init(&raw_empty[s], kWgXpose);   // every transpose thread
     }
-  };
-
-  float acc[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-  const int wg = threadIdx.x >> 7;
-  if (nch > 0) {
-    load(0);
-    store(0);
+    for (int s = 0; s < NO; ++s) {
+      mbar_init(&op_full[s], kWgXpose);
+      mbar_init(&op_empty[s], 8);       // one lane of each MMA warp
+    }
+    fence_mbar_init();
   }
-  fence_proxy_async_smem();
   __syncthreads();
-  for (int c = 0; c < nch; ++c) {
-    const uint32_t st = smem_u32(smem + (c & 1) * Cfg::kStage);
-    const uint32_t a0 = st + wg * 64 * 128;                       // this warpgroup's 64 rows of the A tile
-    const uint32_t b0 = diag ? st : st + Cfg::kOps * kWgTile;     // a diagonal tile multiplies A by itself
-    wgmma_fence();
+
+  if (threadIdx.x < kWgXpose) {
+    // ---- TMA issue (thread 0) and transpose warpgroups ----
+    setmaxnreg_dec<80>();
+    const int m = threadIdx.x % kBlk, h = threadIdx.x / kBlk;   // column, parity of its 4-sample groups
+    const CUtensorMap* mapA = &p.map[p.blk_view[bi]];
+    const CUtensorMap* mapB = &p.map[p.blk_view[bj]];
+    const int colA = p.blk_col0[bi], colB = p.blk_col0[bj];
+    auto issue = [&](int c) {
+      const int s = c % NR;
+      const int row = (int)(p.row_base + r0 + (int64_t)c * kWgKC);
+      mbar_arrive_expect_tx(&raw_full[s], diag ? kWgTile : 2 * kWgTile);
+      tma_load_2d(raw + s * Cfg::kRawStage, mapA, &raw_full[s], colA, row);
+      if (!diag) tma_load_2d(raw + s * Cfg::kRawStage + kWgTile, mapB, &raw_full[s], colB, row);
+    };
+    if (threadIdx.x == 0)
+      for (int c = 0; c < min(NR, nch); ++c) issue(c);
+
+    float csum = 0.f;   // column m of a diagonal tile over the 4-sample groups of parity h
+    auto transpose = [&](const float* src, uint8_t* hi, uint8_t* lo, bool sums) {
 #pragma unroll
-    for (int kk = 0; kk < kWgKC / 8; ++kk) {
-      const uint64_t a_hi = wgmma_desc_k128(a0 + 32 * kk), b_hi = wgmma_desc_k128(b0 + 32 * kk);
-      if (X3) {
-        const uint64_t a_lo = wgmma_desc_k128(a0 + kWgTile + 32 * kk), b_lo = wgmma_desc_k128(b0 + kWgTile + 32 * kk);
-        wgmma_tf32<128>(acc, a_lo, b_hi);   // small cross terms first
-        wgmma_tf32<128>(acc, a_hi, b_lo);
+      for (int j = 0; j < kWgKC / 8; ++j) {
+        const int kg = 2 * j + h;
+        float v[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[e] = src[(4 * kg + e) * kBlk + m];   // lanes walk columns: conflict-free
+        const uint32_t off = k128_offset(m, kg);
+        *reinterpret_cast<float4*>(hi + off) = make_float4(tf32_hi(v[0]), tf32_hi(v[1]), tf32_hi(v[2]), tf32_hi(v[3]));
+        if (X3)
+          *reinterpret_cast<float4*>(lo + off) = make_float4(tf32_residual(v[0]), tf32_residual(v[1]),
+                                                             tf32_residual(v[2]), tf32_residual(v[3]));
+        if (sums) csum += (v[0] + v[1]) + (v[2] + v[3]);
       }
-      wgmma_tf32<128>(acc, a_hi, b_hi);
+    };
+    for (int c = 0; c < nch; ++c) {
+      const int sr = c % NR, so = c % NO;
+      mbar_wait(&raw_full[sr], (c / NR) & 1);
+      mbar_wait(&op_empty[so], ((c / NO) & 1) ^ 1);   // the MMAs of slice c - NO have retired
+      const float* src = reinterpret_cast<const float*>(raw + sr * Cfg::kRawStage);
+      uint8_t* dst = ops + so * Cfg::kOpStage;
+      transpose(src, dst, dst + kWgTile, diag);
+      if (!diag) transpose(src + kBlk * kWgKC, dst + Cfg::kOps * kWgTile, dst + (Cfg::kOps + 1) * kWgTile, false);
+      fence_proxy_async_smem();   // the generic-proxy stores become visible to wgmma (async proxy)
+      mbar_arrive(&raw_empty[sr]);
+      mbar_arrive(&op_full[so]);
+      if (threadIdx.x == 0 && c + NR < nch) {
+        mbar_wait(&raw_empty[sr], (c / NR) & 1);
+        issue(c + NR);
+      }
     }
-    wgmma_commit();
-    const bool more = c + 1 < nch;
-    if (more) load(c + 1);
+    if (diag) {   // even + odd groups
+      float* odd = reinterpret_cast<float*>(smem + Cfg::kSumOff);
+      if (h) odd[m] = csum;
+      asm volatile("bar.sync 1, %0;" ::"n"(kWgXpose) : "memory");
+      if (!h) p.partial_sum[(size_t)split * p.Dp + bi * kBlk + m] = csum + odd[m];
+    }
+  } else {
+    // ---- MMA warpgroups ----
+    setmaxnreg_inc<168>();
+    const int wg = (threadIdx.x - kWgXpose) >> 7;
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    wgmma_fence_regs<64>(acc);   // keeps the zeroing out of the wgmma pipeline (else ptxas serialises the wgmmas)
+    for (int c = 0; c < nch; ++c) {
+      const int so = c % NO;
+      mbar_wait(&op_full[so], (c / NO) & 1);
+      const uint32_t st = smem_u32(ops + so * Cfg::kOpStage);
+      const uint32_t a0 = st + wg * 64 * 128;                       // this warpgroup's 64 rows of the A tile
+      const uint32_t b0 = diag ? st : st + Cfg::kOps * kWgTile;     // a diagonal tile multiplies A by itself
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < kWgKC / 8; ++kk) {
+        const uint64_t a_hi = wgmma_desc_k128(a0 + 32 * kk), b_hi = wgmma_desc_k128(b0 + 32 * kk);
+        if (X3) {
+          const uint64_t a_lo = wgmma_desc_k128(a0 + kWgTile + 32 * kk), b_lo = wgmma_desc_k128(b0 + kWgTile + 32 * kk);
+          wgmma_tf32<128>(acc, a_lo, b_hi);   // small cross terms first
+          wgmma_tf32<128>(acc, a_hi, b_lo);
+        }
+        wgmma_tf32<128>(acc, a_hi, b_hi);
+      }
+      wgmma_commit();
+      wgmma_wait_1();   // the MMAs of slice c - 1 have retired: hand their operand stage back
+      if (c > 0 && (threadIdx.x & 31) == 0) mbar_arrive(&op_empty[(c - 1) % NO]);
+    }
     wgmma_wait_all();
     wgmma_fence_regs<64>(acc);
-    if (more) store((c + 1) & 1);   // that stage was last read by the wgmmas of slice c - 1, retired before the barrier
-    fence_proxy_async_smem();
-    __syncthreads();
-  }
 
-  // ---- epilogue: fragments -> partial slab of this split ----
-  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  float* P = p.partial + (size_t)split * p.Dp * p.Dp;
-  const int row0 = bi * kBlk + wg * 64 + warp * 16 + (lane >> 2);
-  const int col0 = bj * kBlk + 2 * (lane & 3);
+    // ---- epilogue: fragments -> partial slab of this split ----
+    const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    float* P = p.partial + (size_t)split * p.Dp * p.Dp;
+    const int row0 = bi * kBlk + wg * 64 + warp * 16 + (lane >> 2);
+    const int col0 = bj * kBlk + 2 * (lane & 3);
 #pragma unroll
-  for (int r = 0; r < 64; r += 2) {
-    const int row = row0 + 8 * ((r >> 1) & 1), col = col0 + 8 * (r >> 2);
-    *reinterpret_cast<float2*>(P + (size_t)row * p.Dp + col) = make_float2(acc[r], acc[r + 1]);
-  }
-  if (diag) {
-    if (threadIdx.x >= kBlk) colsum_hi[threadIdx.x - kBlk] = csum;
-    __syncthreads();
-    if (threadIdx.x < kBlk)
-      p.partial_sum[(size_t)split * p.Dp + bi * kBlk + threadIdx.x] = csum + colsum_hi[threadIdx.x];
+    for (int r = 0; r < 64; r += 2) {
+      const int row = row0 + 8 * ((r >> 1) & 1), col = col0 + 8 * (r >> 2);
+      *reinterpret_cast<float2*>(P + (size_t)row * p.Dp + col) = make_float2(acc[r], acc[r + 1]);
+    }
   }
 }
 // =============================================================================================
@@ -549,30 +607,88 @@ size_t moments_workspace_bytes(int dtype, int precision, const ColumnLayout& L, 
 }
 
 namespace {
-int moments_tf32_pass(const ColumnLayout& L, const void* const* views, const int64_t* lds, int64_t n_rows, int mode,
-                      double* moments_out, void* ws, size_t ws_bytes, cudaStream_t stream, int accumulate);
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// cuTensorMapEncodeTiled through the runtime's driver entry point (no link against libcuda)
+EncodeTiledFn encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(f);
+  });
+  return fn;
 }
+
+// Row-major fp32 view (n_rows x d, row pitch ld floats) read in [32 rows x 128 columns] boxes, unswizzled; elements
+// past column d or row n_rows read as zero.
+int encode_view_map(CUtensorMap* map, const void* ptr, int64_t n_rows, int64_t d, int64_t ld) {
+  EncodeTiledFn enc = encode_fn();
+  if (!enc) {
+    set_error("cuTensorMapEncodeTiled entry point not available (driver too old?)");
+    return -2;
+  }
+  cuuint64_t gdim[2] = {(cuuint64_t)d, (cuuint64_t)n_rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)ld * 4};
+  cuuint32_t box[2] = {(cuuint32_t)kBlk, (cuuint32_t)kWgKC};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed with CUresult %d (d=%lld n=%lld ld=%lld)", (int)r, (long long)d,
+              (long long)n_rows, (long long)ld);
+    return -3;
+  }
+  return 0;
+}
+
+int moments_tf32_pass(const ColumnLayout& L, WgParams& prm, int64_t row_base, int64_t n_rows, int mode,
+                      double* moments_out, void* ws, size_t ws_bytes, cudaStream_t stream, int accumulate);
+
+}  // namespace
 
 // The 3xTF32 modes bound one accumulator run to 2048 samples (plan_tc) and the split partials to 2 GiB: inputs longer
 // than tc_rows_cap() rows are processed in equal passes whose float64 moments add up in moments_out (the moments are
-// additive over rows; operands and partials are sized for one pass).
+// additive over rows; partials are sized for one pass).  The tensor maps span all rows; a pass offsets the row
+// coordinate.
 int moments_tf32(const ColumnLayout& L, const void* const* views, const int64_t* lds, int64_t n_rows, int mode,
                  double* moments_out, void* ws, size_t ws_bytes, cudaStream_t stream) {
   CCAB_CHECK_ARG(n_rows >= 1 && n_rows < (int64_t)1 << 31, "n_rows out of range");
+  for (int v = 0; v < L.n_views; ++v)
+    CCAB_CHECK_ARG((reinterpret_cast<uintptr_t>(views[v]) & 15) == 0 && lds[v] % 4 == 0,
+                   "TF32 moments need 16-byte aligned views and lds %% 4 == 0 (view %d: ld %lld)", v,
+                   (long long)lds[v]);
   {
-    int dev = 0;   // bind the primary context to this thread before the driver-API tensor-map encoder (see tgemm.cu)
+    int dev = 0;   // bind the primary context to this thread before the driver-API tensor-map encoder
     CCAB_CUDA(cudaGetDevice(&dev));
     CCAB_CUDA(cudaSetDevice(dev));
   }
+  WgParams prm;
+  memset(&prm, 0, sizeof(prm));
+  for (int v = 0; v < L.n_views; ++v) {
+    int rc = encode_view_map(&prm.map[v], views[v], n_rows, L.dims[v], lds[v]);
+    if (rc) return rc;
+  }
+  int b = 0;
+  for (int v = 0; v < L.n_views; ++v)
+    for (int c = 0; c < L.dims[v]; c += kBlk, ++b) {
+      prm.blk_view[b] = (uint8_t)v;
+      prm.blk_col0[b] = c;
+    }
   const int64_t cap = tc_rows_cap(L, mode);
-  if (n_rows <= cap) return moments_tf32_pass(L, views, lds, n_rows, mode, moments_out, ws, ws_bytes, stream, 0);
+  if (n_rows <= cap) return moments_tf32_pass(L, prm, 0, n_rows, mode, moments_out, ws, ws_bytes, stream, 0);
   const int64_t npass = ceil_div(n_rows, cap);
   const int64_t per = std::min(cap, ceil_div(ceil_div(n_rows, npass), 2048) * 2048);
   int pass = 0;
   for (int64_t r0 = 0; r0 < n_rows; r0 += per, ++pass) {
-    const void* sub[kMaxViews];
-    for (int v = 0; v < L.n_views; ++v) sub[v] = static_cast<const float*>(views[v]) + r0 * lds[v];
-    int rc = moments_tf32_pass(L, sub, lds, std::min(per, n_rows - r0), mode, moments_out, ws, ws_bytes, stream,
+    int rc = moments_tf32_pass(L, prm, r0, std::min(per, n_rows - r0), mode, moments_out, ws, ws_bytes, stream,
                                pass > 0);
     if (rc) return rc;
   }
@@ -580,7 +696,9 @@ int moments_tf32(const ColumnLayout& L, const void* const* views, const int64_t*
 }
 
 namespace {
-int moments_tf32_pass(const ColumnLayout& L, const void* const* views, const int64_t* lds, int64_t n_rows, int mode,
+// One pass over rows [row_base, row_base + n_rows).  Its splits end on multiples of 32 rows from row_base, and a pass
+// that is not the last ends on a multiple of 2048, so no slice reads rows of the next pass.
+int moments_tf32_pass(const ColumnLayout& L, WgParams& prm, int64_t row_base, int64_t n_rows, int mode,
                       double* moments_out, void* ws, size_t ws_bytes, cudaStream_t stream, int accumulate) {
   TcPlan P = plan_tc(L, n_rows, mode);
   const size_t need = align256(P.partial_bytes) + align256(P.sum_bytes) + 256;
@@ -589,23 +707,11 @@ int moments_tf32_pass(const ColumnLayout& L, const void* const* views, const int
   float* d_partial = reinterpret_cast<float*>(w);
   float* d_partial_sum = reinterpret_cast<float*>(w + align256(P.partial_bytes));
 
-  WgParams prm;
-  memset(&prm, 0, sizeof(prm));
-  for (int v = 0; v < L.n_views; ++v) {
-    prm.view_ptr[v] = static_cast<const float*>(views[v]);
-    prm.view_ld[v] = lds[v];
-    prm.view_dim[v] = L.dims[v];
-  }
-  int b = 0;
-  for (int v = 0; v < L.n_views; ++v)
-    for (int c = 0; c < L.dims[v]; c += kBlk, ++b) {
-      prm.blk_view[b] = (uint8_t)v;
-      prm.blk_col0[b] = c;
-    }
   prm.partial = d_partial;
   prm.partial_sum = d_partial_sum;
   prm.n_rows = n_rows;
   prm.rows_per_split = (int64_t)P.chunks_per_split * kWgKC;
+  prm.row_base = row_base;
   prm.nblocks = L.nblocks;
   prm.Dp = L.Dp;
   dim3 grid(P.ntiles, P.num_splits);

@@ -52,7 +52,8 @@ int64_t ccab_launch_count(void);
  * np.cov(...) cca_zoo/linear/_mcca.py:150-152,166 and cca_zoo/linear/_gcca.py:101,
  * z.T @ z cca_zoo/deep/objectives.py:86-92; the column sums replace v.mean(axis=0) cca_zoo/_base.py:97.
  * views[v]: device pointer to an n_rows x dims[v] row-major array with leading dimension lds[v]
- * (TF32 paths need 16-byte aligned pointers and lds[v] % 4 == 0). */
+ * (TF32 paths read the views with TMA: they need 16-byte aligned pointers and lds[v] % 4 == 0, and return -1
+ * otherwise). */
 int64_t ccab_moments_size(int n_views, const int64_t* dims);
 int64_t ccab_moments_padded_dim(int n_views, const int64_t* dims);
 size_t ccab_moments_workspace_bytes(int dtype, int precision, int n_views, const int64_t* dims, int64_t n_rows);
