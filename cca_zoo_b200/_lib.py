@@ -54,7 +54,6 @@ SIGNATURES = {
                                    C.c_double, C.c_int, C.c_double, _vp, C.c_int64, _vp, _vp, _vp]),
     "ccab_ccaloss_small": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, C.c_double, _vp, _vp, _vp, _vp, _vp,
                                      _vp]),
-    "ccab_potrf": (C.c_int, [C.c_int, C.c_int, _vp, C.c_int64, C.c_double, _vp, _vp]),
     "ccab_potrf_inv_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "ccab_potrf_inv": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int64,
                                  C.c_double, _vp, _vp, C.c_size_t, _vp]),
@@ -71,14 +70,12 @@ SIGNATURES = {
     "ccab_mcca_fit_result_layout": (C.c_int, [C.c_int, C.c_int, _i64p, C.c_int, C.c_int, _i64p]),
     "ccab_mcca_fit": (C.c_int, [C.c_int, C.c_int, _i64p, _vp, _vp, C.c_double, C.c_int, C.POINTER(C.c_double),
                                 C.c_double, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp, C.c_size_t, _vp]),
-    "ccab_trsm": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp]),
     "ccab_scale": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int64,
                              _vp]),
     "ccab_center_columns": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp]),
     "ccab_frobenius_norm": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp, _vp]),
     "ccab_profile_moments": (C.c_int, [C.c_int]),
     "ccab_profile_moments_last_ms": (C.c_double, []),
-    "ccab_debug_set": (C.c_int, [C.c_char_p, C.c_int]),
 }
 
 _lib = None

@@ -26,7 +26,7 @@ def _eps(dtype):
 
 class _two_streams:
     """Fork the current stream into two side streams and join them back on exit: independent per-view
-    chains of small latency-bound kernels (Cholesky factorisations, back-substitutions) overlap."""
+    chains of small latency-bound kernels (Cholesky factorisations and inverses) overlap."""
 
     _pool = {}
 
@@ -98,14 +98,14 @@ def _block_eigh(C, dims):
     return lams, vts
 
 
-def _cholqr_(Y, flags, passes=1):
-    """Orthonormalise the columns of Y (n x p) in place by CholQR (Gram matrix, Cholesky, triangular solve).
+def _cholqr(Y, flags, passes=1):
+    """Orthonormalise the columns of Y (n x p) by CholQR: G = Y^T Y = L L^T, returns Y L^-T.
     The device-side Cholesky status flags are appended to ``flags`` (checked once, later, by the caller):
     a non-zero flag means the block lost rank."""
     for _ in range(passes):
-        G = ops.gemm(Y, Y, transa=True)
-        flags.append(ops.potrf_(G))
-        ops.trsm_(G, Y, side="right", trans=True)
+        Ginv, info = ops.potrf_inv_(ops.gemm(Y, Y, transa=True))
+        flags.append(info)
+        Y = ops.gemm(Y, Ginv, transb=True)
     return Y
 
 
@@ -135,7 +135,7 @@ def topk_svd(T, k, max_rounds=4, iters_per_round=5, oversample=None, seed=1234):
             # one application of T^T T between orthonormalisations: the block's condition number grows by
             # (sigma_1/sigma_p)^2 per step, far below what a single CholQR pass tolerates
             Y = ops.gemm(T, Z)                                    # d1 x p
-            Z = _cholqr_(ops.gemm(T, Y, transa=True), flags,      # d2 x p
+            Z = _cholqr(ops.gemm(T, Y, transa=True), flags,       # d2 x p
                          passes=2 if it == iters_per_round - 1 else 1)
         # Rayleigh-Ritz on Y = T Z (d1 x p): Y^T Y = Vy diag(sig^2) Vy^T (p x p Jacobi eigensolve; the block is
         # well conditioned -- sigma_1/sigma_p is a few units -- so squaring costs nothing at the top), then
@@ -171,14 +171,14 @@ def topk_eigsh(K, k, shift, max_rounds=6, iters_per_round=8, seed=4321):
     gen = torch.Generator(device=K.device).manual_seed(seed)
     Z = torch.randn((D, p), generator=gen, device=K.device, dtype=K.dtype)
     flags = []
-    _cholqr_(Z, flags, passes=2)
+    Z = _cholqr(Z, flags, passes=2)
     tol = 200.0 * _eps(K.dtype)
     for _ in range(max_rounds):
         for it in range(iters_per_round):
             Y = ops.gemm(K, Z)
             if shift != 0.0:
                 Y.add_(Z, alpha=shift)
-            Z = _cholqr_(Y, flags, passes=2 if it == iters_per_round - 1 else 1)
+            Z = _cholqr(Y, flags, passes=2 if it == iters_per_round - 1 else 1)
         KZ = ops.gemm(K, Z)                                   # D x p
         H = ops.gemm(Z, KZ, transa=True)                      # p x p Rayleigh quotient matrix
         H = 0.5 * (H + H.T)
@@ -211,11 +211,10 @@ def _cholesky_whiteners(C, dims, c, scales, eps_floor):
         R = (1.0 - c[i]) * C[s, s]
         R.diagonal().add_(c[i])
         dmax = R.diagonal().max()
-        flags.append(ops.potrf_(R, pivot_tol=0.0))
-        Linv = torch.eye(dims[i], dtype=C.dtype, device=C.device)
-        ops.trsm_(R, Linv, side="left")
+        Linv, info = ops.potrf_inv_(R, pivot_tol=0.0)
+        flags.append(info)
         norms.append(torch.stack([ops.frobenius_norm(Linv)[0], dmax]))
-        out.append((R, Linv))
+        out.append(Linv)
     stats = torch.cat([torch.stack(flags).max().to(C.dtype).reshape(1), torch.stack(norms).reshape(-1)]).cpu()
     if float(stats[0]) != 0.0:
         return None
@@ -226,7 +225,7 @@ def _cholesky_whiteners(C, dims, c, scales, eps_floor):
         lam_min_lb = 1.0 / (fro * fro)
         if lam_min_lb < eps_floor or lam_min_lb < _rank_tol(dims[i], C.dtype) * dmax:
             return None
-    return [Linv if scales[i] == 1.0 else Linv.mul_(scales[i] ** 0.5) for i, (_, Linv) in enumerate(out)]
+    return [Linv if scales[i] == 1.0 else Linv.mul_(scales[i] ** 0.5) for i, Linv in enumerate(out)]
 
 
 def mcca_weights_cholesky(C, dims, latent_dimensions, c, eps):
@@ -326,12 +325,12 @@ def rcca_weights_cholesky(C, dims, n_samples, latent_dimensions, c):
                 R = (1.0 - c[i]) * C[s, s]
                 R.diagonal().add_(c[i])
                 tol = _rank_tol(dims[i], C.dtype) * ((1.0 - c[i]) * float(dmax[i]) + c[i])
-                infos.append(ops.potrf_(R, pivot_tol=tol))
-                # explicit L^-1 (one triangular solve against I): everything downstream -- T and the
-                # back-substitution of the k weight vectors -- becomes plain GEMMs.  R is ridge-regularised
-                # and certified positive definite, so cond(L) = sqrt(cond(R)) is benign.
-                E = torch.eye(dims[i], dtype=C.dtype, device=C.device)
-                Linv.append(ops.trsm_(R, E, side="left"))
+                # explicit L^-1: everything downstream -- T and the back-substitution of the k weight vectors --
+                # becomes plain GEMMs.  R is ridge-regularised and certified positive definite, so
+                # cond(L) = sqrt(cond(R)) is benign.
+                Li, info = ops.potrf_inv_(R, pivot_tol=tol)
+                Linv.append(Li)
+                infos.append(info)
     if int(torch.stack(infos).max().item()) != 0:
         return None
     T = ops.gemm(ops.gemm(Linv[0], C[s1, s2]), Linv[1], transb=True)      # L1^-1 C12 L2^-T

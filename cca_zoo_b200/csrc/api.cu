@@ -8,7 +8,6 @@
 #include <exception>
 
 #include "ccaloss.cuh"
-#include "chol.cuh"
 #include "cholinv.cuh"
 #include "common.cuh"
 #include "dense.cuh"
@@ -439,18 +438,6 @@ int ccab_ccaloss_small(int dtype, int d1, int d2, const void* C, int64_t ldc, do
   CCAB_CATCH
 }
 
-int ccab_potrf(int dtype, int n, void* A, int64_t lda, double pivot_tol, int* info_dev, void* stream) {
-  CCAB_TRY
-  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
-  CCAB_CHECK_ARG(A && info_dev, "null pointer argument");
-  int rc = require_device();
-  if (rc) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (dtype == CCAB_F32) return potrf<float>(n, static_cast<float*>(A), lda, pivot_tol, info_dev, s);
-  return potrf<double>(n, static_cast<double*>(A), lda, pivot_tol, info_dev, s);
-  CCAB_CATCH
-}
-
 size_t ccab_potrf_inv_workspace_bytes(int dtype, int n, int batch) {
   if (n < 1 || batch < 1) return 0;
   return dtype == CCAB_F32 ? potrf_inv_workspace_bytes<float>(n, batch) : potrf_inv_workspace_bytes<double>(n, batch);
@@ -470,26 +457,6 @@ int ccab_potrf_inv(int dtype, int n, int batch, void* A, int64_t lda, int64_t st
                             pivot_tol, nullptr, info_dev, workspace, workspace_bytes, s);
   return potrf_inv<double>(n, batch, static_cast<double*>(A), lda, stride_a, static_cast<double*>(Linv), ldi, stride_i,
                            pivot_tol, nullptr, info_dev, workspace, workspace_bytes, s);
-  CCAB_CATCH
-}
-
-int ccab_trsm(int dtype, int side, int trans, int n, int m, const void* L, int64_t ldl, void* B, int64_t ldb,
-              void* stream) {
-  CCAB_TRY
-  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
-  CCAB_CHECK_ARG(L && B, "null pointer argument");
-  CCAB_CHECK_ARG(side == 0 || (side == 1 && trans == 1), "supported: left (trans 0/1) and right with trans=1");
-  int rc = require_device();
-  if (rc) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (side == 0) {
-    if (dtype == CCAB_F32)
-      return trsm_left<float>(trans, n, m, static_cast<const float*>(L), ldl, static_cast<float*>(B), ldb, s);
-    return trsm_left<double>(trans, n, m, static_cast<const double*>(L), ldl, static_cast<double*>(B), ldb, s);
-  }
-  if (dtype == CCAB_F32)
-    return trsm_right_lt<float>(n, m, static_cast<const float*>(L), ldl, static_cast<float*>(B), ldb, s);
-  return trsm_right_lt<double>(n, m, static_cast<const double*>(L), ldl, static_cast<double*>(B), ldb, s);
   CCAB_CATCH
 }
 
@@ -665,21 +632,5 @@ int ccab_profile_moments(int enable) {
   return 0;
 }
 double ccab_profile_moments_last_ms(void) { return (double)moments_profile_last_ms(); }
-
-int ccab_debug_set(const char* key, int value) {
-  if (!key) return -1;
-  TcDebug& d = tc_debug();
-  if (!strcmp(key, "force_splits")) d.force_splits = value;
-  else if (!strcmp(key, "f64_simt")) d.f64_simt = value < 0 ? 0 : value;
-  else if (!strcmp(key, "gemm_force_fma")) xgemm_force_fma() = value < 0 ? 0 : value;
-  else if (!strcmp(key, "gemm_split")) xgemm_split_enabled() = value < 0 ? 1 : value;
-  else if (!strcmp(key, "jacobi_inner_sweeps")) jacobi_inner_sweeps() = value;
-  else if (!strcmp(key, "jacobi_force_unfused")) jacobi_force_unfused() = value;
-  else {
-    set_error("unknown debug key %s", key);
-    return -1;
-  }
-  return 0;
-}
 
 }  // extern "C"

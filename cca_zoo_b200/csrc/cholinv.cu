@@ -357,7 +357,7 @@ int potrf_inv(int n, int batch, T* A, int64_t lda, int64_t strideA, T* Linv, int
 // a scratch copy.
 template <typename T>
 int potrf_panel_gemm(const GemmArgs<T>& g, T* scratch, int64_t strideScratch, cudaStream_t stream) {
-  if (std::is_same<T, float>::value && !xgemm_force_fma() && g.n <= 128) {
+  if (std::is_same<T, float>::value && g.n <= 128) {
     TgemmArgs a;
     a.transa = g.transa; a.transb = g.transb; a.m = g.m; a.n = g.n; a.k = g.k;
     a.A = reinterpret_cast<const float*>(g.A); a.lda = g.lda; a.strideA = g.strideA;

@@ -111,19 +111,6 @@ int gemm_fma(const GemmArgs<T>& g, cudaStream_t stream) {
 template int gemm_fma<float>(const GemmArgs<float>&, cudaStream_t);
 template int gemm_fma<double>(const GemmArgs<double>&, cudaStream_t);
 
-template <typename T>
-int gemm(int transa, int transb, int m, int n, int k, T alpha, const T* A, int64_t lda, const T* B, int64_t ldb,
-         T beta, T* C, int64_t ldc, cudaStream_t stream) {
-  GemmArgs<T> g;
-  g.transa = transa; g.transb = transb; g.m = m; g.n = n; g.k = k; g.alpha = alpha; g.beta = beta;
-  g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc;
-  return gemm_fma<T>(g, stream);
-}
-template int gemm<float>(int, int, int, int, int, float, const float*, int64_t, const float*, int64_t, float, float*,
-                         int64_t, cudaStream_t);
-template int gemm<double>(int, int, int, int, int, double, const double*, int64_t, const double*, int64_t, double,
-                          double*, int64_t, cudaStream_t);
-
 // ---------------------------------------------------------------------------------------------------------------
 // float64 GEMM on the fp64 tensor pipe: mma.sync.aligned.m8n8k4.f64 (DMMA; tcgen05 has no f64 kind).  64 x 64 output
 // tile, 8 warps x (4 x 2) m8n8 fragments, 16-deep k chunks staged through skewed shared tiles ([k][64 + 8] doubles:
@@ -345,13 +332,13 @@ int xgemm<float>(const GemmArgs<float>& g, cudaStream_t stream) {
   a.Ct = g.Ct; a.ldct = g.ldct; a.strideCt = g.strideCt; a.strideCt2 = g.strideCt2;
   a.batch = g.batch; a.batch2 = g.batch2; a.lower_only = g.lower_only;
   const bool big = (int64_t)g.m * g.n * g.k >= ((int64_t)1 << 21) && g.k >= 16;   // >= 128^3: the pipeline fill (~9 us) pays off
-  if (big && !xgemm_force_fma() && tgemm_supported(a)) {
+  if (big && tgemm_supported(a)) {
     // thin products (few 128 x 64 output tiles, long reduction) occupy a handful of SMs for k / 32 pipeline steps:
     // when the caller lends scratch, run equal k-slices as a batch and add the partial tiles in slice order
     // (deterministic).  Slices along a K-major operand overlap in memory (batch stride < row stride), which TMA
     // tensor maps allow; should the encoder refuse, the unsplit product below still runs.
     const int64_t tiles = ceil_div(g.m, 128) * ceil_div(g.n, 64);
-    if (g.splitk_ws && xgemm_split_enabled() && g.batch == 1 && g.batch2 == 1 && !g.lower_only && tiles <= 24 && g.k >= 512) {
+    if (g.splitk_ws && g.batch == 1 && g.batch2 == 1 && !g.lower_only && tiles <= 24 && g.k >= 512) {
       int ns = (int)std::min<int64_t>(std::min<int64_t>(8, 148 / tiles), g.k / 128);
       while (ns >= 2 && (g.k % ns != 0 || (g.k / ns) % 32 != 0)) --ns;
       const int64_t ldp = ceil_div(g.n, 4) * 4;
@@ -381,16 +368,8 @@ int xgemm<float>(const GemmArgs<float>& g, cudaStream_t stream) {
 }
 template <>
 int xgemm<double>(const GemmArgs<double>& g, cudaStream_t stream) {
-  if (!xgemm_force_fma() && g.k >= 8) return gemm_dmma(g, stream);   // fp64 tensor pipe (DMMA)
+  if (g.k >= 8) return gemm_dmma(g, stream);   // fp64 tensor pipe (DMMA)
   return gemm_fma<double>(g, stream);
-}
-int& xgemm_force_fma() {
-  static int v = 0;
-  return v;
-}
-int& xgemm_split_enabled() {
-  static int v = 1;
-  return v;
 }
 
 template <typename T>

@@ -30,13 +30,6 @@ template <typename T>
 int gemm_fma(const GemmArgs<T>& g, cudaStream_t stream);   // exact FMA tiles on the CUDA cores
 template <typename T>
 int xgemm(const GemmArgs<T>& g, cudaStream_t stream);      // float: tcgen05 when TMA-addressable, else gemm_fma
-int& xgemm_force_fma();                                    // debug knob: 1 = never use the tensor pipe
-int& xgemm_split_enabled();                                // debug knob: 0 = never split thin float32 products over k
-
-// C (m x n, row-major, ldc) = alpha * op(A) * op(B) + beta * C ; op(X) = X or X^T, row-major storage.
-template <typename T>
-int gemm(int transa, int transb, int m, int n, int k, T alpha, const T* A, int64_t lda, const T* B, int64_t ldb,
-         T beta, T* C, int64_t ldc, cudaStream_t stream);
 
 // Whitening factors from an eigendecomposition (covariance form of svd_whiten,
 // cca_zoo/_utils/_linalg.py:30-38):  for eigenpair j (descending, rows of Vt)

@@ -65,11 +65,6 @@ float moments_profile_last_ms() {
   return ms;
 }
 
-TcDebug& tc_debug() {
-  static TcDebug d = {0, 0};
-  return d;
-}
-
 // =============================================================================================
 // wgmma kernel
 // =============================================================================================
@@ -344,7 +339,7 @@ __global__ void __launch_bounds__(256) moments_simt_kernel(const SimtParams p) {
 
 // =============================================================================================
 // fp64 tensor-core variant of the exact kernel: mma.sync.aligned.m8n8k4.row.col.f64 (DMMA; wgmma has no
-// f64 kind).  Same 64x64 tiles, same partial layout and split planning as moments_simt_kernel<double>.
+// f64 kind).  Same 64x64 tiles, same partial layout and split planning as moments_simt_kernel.
 // 8 warps; warp w owns the 32 x 16 sub-tile (rows 32*(w&1), cols 16*(w>>1)) = 4 x 2 m8n8 fragments.
 // Shared tiles are [k][64 + 8] doubles: the 16-bank skew between consecutive k rows makes the 64-bit
 // fragment loads conflict-free (two wavefronts, the minimum for 32 lanes x 8 bytes).
@@ -556,7 +551,6 @@ TcPlan plan_tc(const ColumnLayout& L, int64_t n_rows, int mode) {
   const int64_t slab = (int64_t)L.Dp * L.Dp * (int64_t)sizeof(float);
   max_splits = (int)std::max<int64_t>(1, std::min<int64_t>(max_splits, ((int64_t)2 << 30) / slab));
   S = std::min(S, max_splits);
-  if (tc_debug().force_splits > 0) S = tc_debug().force_splits;
   S = std::max(1, std::min(S, P.total_chunks));
   P.chunks_per_split = (int)ceil_div(P.total_chunks, S);
   P.num_splits = (int)ceil_div(P.total_chunks, P.chunks_per_split);
@@ -769,7 +763,7 @@ int moments_simt(const ColumnLayout& L, const void* const* views, const int64_t*
   // partial sums of non-diagonal 64-blocks inside a 128-block are never written by the kernel: the
   // reducer only reads what a tile wrote (block-triangle test at 64 granularity).
   dim3 grid(P.ntiles, P.num_splits);
-  if (std::is_same<T, double>::value && !tc_debug().f64_simt)
+  if constexpr (std::is_same<T, double>::value)
     moments_dmma_kernel<<<grid, 256, 0, stream>>>(prm);
   else
     moments_simt_kernel<T><<<grid, 256, 0, stream>>>(prm);

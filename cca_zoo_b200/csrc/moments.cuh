@@ -63,13 +63,6 @@ int moments_exchange_nvls(const ColumnLayout& L, double* moments, double n_local
                           double* sym_multicast, void* const* pads_dev, int rank, int world, int pad_slots,
                           int64_t sym_doubles, unsigned epoch, double* n_total_out, cudaStream_t stream);
 
-// debug knobs of the moment kernels
-struct TcDebug {
-  int force_splits; // <=0: heuristic
-  int f64_simt;     // float64 inputs: 0 = DMMA kernel (default), 1 = CUDA-core FMA kernel
-};
-TcDebug& tc_debug();
-
 // CUDA-event timing of the tensor-core moment kernel launch alone (for bench.py's roofline line)
 void moments_profile_enable(int on);
 float moments_profile_last_ms();

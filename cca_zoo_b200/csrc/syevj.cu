@@ -94,13 +94,13 @@ __device__ __forceinline__ void jacobi_cs(double app, double aqq, double apq, do
   rotated = true;
 }
 
-// Parallel cyclic two-sided Jacobi on a 32 x 32 symmetric matrix in shared memory, 256 threads.
+// One sweep of parallel cyclic two-sided Jacobi on a 32 x 32 symmetric matrix in shared memory, 256 threads.
 // Thread (i, j) owns the 2x2 block of rotation pairs (i, j) in each of the 31 tournament steps; lanes
 // 0..15 of every warp each compute the rotation of pair `lane` once and the warp shares them by shuffle.
 // Wa/Wb: ping-pong copies (stride 33), Q: accumulated rotations (stride 33, starts as I), pairs: the
-// (S-1) x 16 tournament table.  Returns the buffer holding the (nearly) diagonal result.
+// (S-1) x 16 tournament table.  Returns the buffer holding the rotated matrix.
 template <typename T, int S>
-__device__ T* small_syevj(T* Wa, T* Wb, T* Q, const uchar2* pairs, int max_sweeps) {
+__device__ T* small_syevj(T* Wa, T* Wb, T* Q, const uchar2* pairs) {
   static_assert(S == 32, "the thread mapping below is written for 32 x 32 panels and 256 threads");
   constexpr int H = S / 2;
   constexpr int SP = S + 1;
@@ -109,43 +109,39 @@ __device__ T* small_syevj(T* Wa, T* Wb, T* Q, const uchar2* pairs, int max_sweep
   const int i = 2 * warp + (lane >> 4);
   T* cur = Wa;
   T* nxt = Wb;
-  for (int sweep = 0; sweep < max_sweeps; ++sweep) {
-    int any = 0;
-    for (int step = 0; step < S - 1; ++step) {
-      const uchar2 pq = pairs[step * H + j];
-      const int pj = pq.x, qj = pq.y;
-      T cj, sj;
-      bool rj = false;
-      jacobi_cs(cur[pj * SP + pj], cur[qj * SP + qj], cur[pj * SP + qj], cj, sj, rj);
-      const T ci = __shfl_sync(0xffffffffu, cj, i);
-      const T si = __shfl_sync(0xffffffffu, sj, i);
-      const int pi = __shfl_sync(0xffffffffu, pj, i);
-      const int qi = __shfl_sync(0xffffffffu, qj, i);
-      const bool ri = __shfl_sync(0xffffffffu, (int)rj, i) != 0;
-      const T x00 = cur[pi * SP + pj], x01 = cur[pi * SP + qj];
-      const T x10 = cur[qi * SP + pj], x11 = cur[qi * SP + qj];
-      const T y00 = cj * x00 - sj * x01, y01 = sj * x00 + cj * x01;
-      const T y10 = cj * x10 - sj * x11, y11 = sj * x10 + cj * x11;
-      T z00 = ci * y00 - si * y10, z10 = si * y00 + ci * y10;
-      T z01 = ci * y01 - si * y11, z11 = si * y01 + ci * y11;
-      if (i == j && ri) { z01 = T(0); z10 = T(0); }
-      nxt[pi * SP + pj] = z00;
-      nxt[pi * SP + qj] = z01;
-      nxt[qi * SP + pj] = z10;
-      nxt[qi * SP + qj] = z11;
-      if (ri) {  // Q <- Q J_i for rows j and j+H (each (row, pair) owned by exactly one thread)
+  for (int step = 0; step < S - 1; ++step) {
+    const uchar2 pq = pairs[step * H + j];
+    const int pj = pq.x, qj = pq.y;
+    T cj, sj;
+    bool rj = false;
+    jacobi_cs(cur[pj * SP + pj], cur[qj * SP + qj], cur[pj * SP + qj], cj, sj, rj);
+    const T ci = __shfl_sync(0xffffffffu, cj, i);
+    const T si = __shfl_sync(0xffffffffu, sj, i);
+    const int pi = __shfl_sync(0xffffffffu, pj, i);
+    const int qi = __shfl_sync(0xffffffffu, qj, i);
+    const bool ri = __shfl_sync(0xffffffffu, (int)rj, i) != 0;
+    const T x00 = cur[pi * SP + pj], x01 = cur[pi * SP + qj];
+    const T x10 = cur[qi * SP + pj], x11 = cur[qi * SP + qj];
+    const T y00 = cj * x00 - sj * x01, y01 = sj * x00 + cj * x01;
+    const T y10 = cj * x10 - sj * x11, y11 = sj * x10 + cj * x11;
+    T z00 = ci * y00 - si * y10, z10 = si * y00 + ci * y10;
+    T z01 = ci * y01 - si * y11, z11 = si * y01 + ci * y11;
+    if (i == j && ri) { z01 = T(0); z10 = T(0); }
+    nxt[pi * SP + pj] = z00;
+    nxt[pi * SP + qj] = z01;
+    nxt[qi * SP + pj] = z10;
+    nxt[qi * SP + qj] = z11;
+    if (ri) {  // Q <- Q J_i for rows j and j+H (each (row, pair) owned by exactly one thread)
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int r = j + hh * H;
-          const T a = Q[r * SP + pi], b = Q[r * SP + qi];
-          Q[r * SP + pi] = ci * a - si * b;
-          Q[r * SP + qi] = si * a + ci * b;
-        }
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = j + hh * H;
+        const T a = Q[r * SP + pi], b = Q[r * SP + qi];
+        Q[r * SP + pi] = ci * a - si * b;
+        Q[r * SP + qi] = si * a + ci * b;
       }
-      any |= __syncthreads_or((ri && i == j) ? 1 : 0);
-      T* tmp = cur; cur = nxt; nxt = tmp;
     }
-    if (!any) break;
+    __syncthreads();
+    T* tmp = cur; cur = nxt; nxt = tmp;
   }
   return cur;
 }
@@ -246,7 +242,7 @@ __device__ void reorthonormalise(T* Q, T* E, T* Qn) {
 }
 
 template <typename T>
-__global__ void __launch_bounds__(256) jacobi_solve_kernel(const JacobiCtx<T> c, T tol, int inner_sweeps) {
+__global__ void __launch_bounds__(256) jacobi_solve_kernel(const JacobiCtx<T> c, T tol) {
   __shared__ T Wa[kS * kSP];
   __shared__ T Wb[kS * kSP];
   __shared__ T Q[kS * kSP];
@@ -289,7 +285,7 @@ __global__ void __launch_bounds__(256) jacobi_solve_kernel(const JacobiCtx<T> c,
   }
   if (ratio <= (float)tol) return;  // panel already orthogonal: Q = I, apply kernel skips it
 
-  T* fin = small_syevj<T, kS>(Wa, Wb, Q, pairs, inner_sweeps);
+  T* fin = small_syevj<T, kS>(Wa, Wb, Q, pairs);
   __syncthreads();
   if (threadIdx.x < kS) {
     const int i = threadIdx.x;
@@ -372,9 +368,8 @@ __global__ void __launch_bounds__(128) jacobi_apply_kernel(const JacobiCtx<T> c,
 namespace cg = cooperative_groups;
 
 template <typename T>
-__global__ void __launch_bounds__(256) jacobi_round_fused_kernel(const JacobiCtx<T> c, int round, T tol,
-                                                                 int inner_sweeps, int cs, int rows_g,
-                                                                 int rows_v) {
+__global__ void __launch_bounds__(256) jacobi_round_fused_kernel(const JacobiCtx<T> c, int round, T tol, int cs,
+                                                                 int rows_g, int rows_v) {
   extern __shared__ __align__(16) unsigned char fused_smem[];
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
@@ -465,7 +460,7 @@ __global__ void __launch_bounds__(256) jacobi_round_fused_kernel(const JacobiCtx
   if (rank == 0 && threadIdx.x == 0) atomicMax(c.stat + b, __float_as_uint(ratio));
   if (ratio <= (float)tol) return;  // uniform over the cluster (identical W everywhere)
 
-  T* fin = small_syevj<T, kS>(Wa, Wb, Q, pairs, inner_sweeps);
+  T* fin = small_syevj<T, kS>(Wa, Wb, Q, pairs);
   __syncthreads();
   if (threadIdx.x < kS) {
     const int i = threadIdx.x;
@@ -674,15 +669,6 @@ static unsigned* pinned_stat_buffer(size_t count) {
   return buf;
 }
 
-int& jacobi_inner_sweeps() {
-  static int v = 0;
-  return v;
-}
-int& jacobi_force_unfused() {
-  static int v = 0;
-  return v;
-}
-
 namespace {
 inline size_t al(size_t x) { return (x + 255) & ~size_t(255); }
 
@@ -764,20 +750,18 @@ int jacobi_solve(const JacobiArgs<T>& a, void* ws, size_t ws_bytes, cudaStream_t
   }
   const T tol = a.tol > 0 ? (T)a.tol : (T)(4.0 * (double)Eps<T>::v * std::sqrt((double)m));
   const int max_sweeps = a.max_sweeps > 0 ? a.max_sweeps : (std::is_same<T, float>::value ? 16 : 24);
-  const int inner_sweeps = jacobi_inner_sweeps() > 0 ? jacobi_inner_sweeps() : 1;
-  // fused cluster path: smallest cluster (<= 8 CTAs) whose row slice fits comfortably in shared memory
+  // fused cluster path: smallest cluster (<= 8 CTAs) whose row slice fits comfortably in shared memory; when none
+  // fits (large m), each round runs as three kernels (gram / solve / apply)
   int cs = 0, rows_g = 0, rows_v = 0;
   size_t fused_bytes = 0;
-  if (!jacobi_force_unfused()) {
-    for (int cand = 1; cand <= 8; cand *= 2) {
-      const int rg = (int)ceil_div(m, cand), rv = (int)ceil_div(P.n_pad, cand);
-      const size_t bytes = fused_smem_bytes<T>(rg + rv);
-      const size_t limit = (size_t)P.npairs * batch * cand >= 296 ? 100 * 1024 : 200 * 1024;
-      if (bytes <= limit) {
-        cs = cand; rows_g = rg; rows_v = rv; fused_bytes = bytes;
-        // prefer more CTAs per pair while the machine is not full
-        if ((size_t)P.npairs * batch * cand >= 148 || cand == 8) break;
-      }
+  for (int cand = 1; cand <= 8; cand *= 2) {
+    const int rg = (int)ceil_div(m, cand), rv = (int)ceil_div(P.n_pad, cand);
+    const size_t bytes = fused_smem_bytes<T>(rg + rv);
+    const size_t limit = (size_t)P.npairs * batch * cand >= 296 ? 100 * 1024 : 200 * 1024;
+    if (bytes <= limit) {
+      cs = cand; rows_g = rg; rows_v = rv; fused_bytes = bytes;
+      // prefer more CTAs per pair while the machine is not full
+      if ((size_t)P.npairs * batch * cand >= 148 || cand == 8) break;
     }
   }
   if (cs) {
@@ -808,13 +792,12 @@ int jacobi_solve(const JacobiArgs<T>& a, void* ws, size_t ws_bytes, cudaStream_t
         attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;
-        cudaError_t le = cudaLaunchKernelEx(&cfg, jacobi_round_fused_kernel<T>, c, r, tol, inner_sweeps, cs, rows_g,
-                                            rows_v);
+        cudaError_t le = cudaLaunchKernelEx(&cfg, jacobi_round_fused_kernel<T>, c, r, tol, cs, rows_g, rows_v);
         if (le != cudaSuccess) { rc = cuda_fail(le, "jacobi_round_fused_kernel launch"); break; }
         count_launches(1);
       } else {
         jacobi_gram_kernel<T><<<dim3(P.npairs, P.R, batch), 256, 0, stream>>>(c, r); count_launches(1);
-        jacobi_solve_kernel<T><<<dim3(P.npairs, batch), 256, 0, stream>>>(c, tol, inner_sweeps); count_launches(1);
+        jacobi_solve_kernel<T><<<dim3(P.npairs, batch), 256, 0, stream>>>(c, tol); count_launches(1);
         jacobi_apply_kernel<T><<<dim3(P.npairs, apply_chunks, batch), 128, 0, stream>>>(c, r); count_launches(1);
       }
     }

@@ -25,11 +25,6 @@ struct JacobiArgs {
   float* final_offdiag;     // host: largest normalised off-diagonal Gram entry of the last sweep
 };
 
-// tuning knob: inner (panel) Jacobi sweeps per block visit; <=0 selects the default
-int& jacobi_inner_sweeps();
-// tuning knob: 1 = always use the three-kernel (gram / solve / apply) round instead of the fused cluster kernel
-int& jacobi_force_unfused();
-
 template <typename T>
 size_t jacobi_workspace_bytes(int m, int n, int batch);
 

@@ -475,19 +475,6 @@ def ccaloss_bwd(z1, z2, saved, grad_out):
     return g1, g2
 
 
-def potrf_(A, pivot_tol=0.0):
-    """In place lower Cholesky of a square row-major CUDA matrix.  Returns the device info flag (int32[1])."""
-    lib = _lib.load()
-    _require_cuda(A, "A")
-    if A.dim() != 2 or A.shape[0] != A.shape[1] or A.stride(1) != 1:
-        raise ValueError("square row-major matrix expected")
-    info = torch.zeros(1, dtype=torch.int32, device=A.device)
-    with torch.cuda.device(A.device):
-        rc = lib.ccab_potrf(_DT[A.dtype], A.shape[0], _ptr(A), A.stride(0), float(pivot_tol), _ptr(info), _stream(A))
-    _lib.check(rc, "ccab_potrf")
-    return info
-
-
 def potrf_inv_(A, pivot_tol=0.0):
     """In place lower Cholesky of A (n x n or batch x n x n, row-major) AND the explicit inverse of the factor.
 
@@ -508,27 +495,6 @@ def potrf_inv_(A, pivot_tol=0.0):
                                 n * n, float(pivot_tol), _ptr(info), _ptr(ws), ws.numel(), _stream(A))
     _lib.check(rc, "ccab_potrf_inv")
     return (Linv[0] if squeeze else Linv), info
-
-
-def trsm_(L, B, side="left", trans=False):
-    """In place triangular solve with the lower factor L: left: B <- L^-1 B / L^-T B; right: B <- B L^-T."""
-    lib = _lib.load()
-    _require_cuda(B, "B")
-    if B.stride(1) != 1 or L.stride(1) != 1:
-        raise ValueError("row-major matrices expected")
-    n = L.shape[0]
-    if side == "left":
-        if B.shape[0] != n:
-            raise ValueError("shape mismatch")
-        args = (0, int(trans), n, B.shape[1])
-    else:
-        if B.shape[1] != n or not trans:
-            raise ValueError("right side supports B <- B L^-T only")
-        args = (1, 1, n, B.shape[0])
-    with torch.cuda.device(B.device):
-        rc = lib.ccab_trsm(_DT[B.dtype], *args, _ptr(L), L.stride(0), _ptr(B), B.stride(0), _stream(B))
-    _lib.check(rc, "ccab_trsm")
-    return B
 
 
 # status bits of the device-side fit (csrc/fit.cuh)
@@ -641,7 +607,3 @@ def frobenius_norm(A):
         rc = lib.ccab_frobenius_norm(_DT[A.dtype], A.shape[0], A.shape[1], _ptr(A), A.stride(0), _ptr(out), _stream(A))
     _lib.check(rc, "ccab_frobenius_norm")
     return out
-
-
-def debug_set(key: str, value: int) -> None:
-    _lib.check(_lib.load().ccab_debug_set(key.encode(), int(value)), "ccab_debug_set")

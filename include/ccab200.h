@@ -195,22 +195,11 @@ int ccab_ccaloss_small(int dtype, int d1, int d2, const void* C, int64_t ldc, do
                        void* P, void* G22, void* min_pivot, void* stream);
 
 /* ---- Cholesky route of the generalised problem ----------------------------------------------------
- * ccab_potrf: lower triangle of A (n x n, row-major, device) <- L with A = L L^T, in place (the strict
- * upper triangle is not referenced).  *info_dev (device int): 0, or the 1-based index of the first pivot
- * <= pivot_tol (matrix not numerically positive definite: callers fall back to the eigen route).
- * ccab_trsm: side 0: B (n x m) <- L^-1 B (trans 0) or L^-T B (trans 1); side 1 (trans must be 1):
- * B (m x n) <- B L^-T.  L is n x n lower triangular.
- * Replaces the Cholesky + back-substitution inside scipy.linalg.eigh(A, B) (LAPACK *sygvx,
- * cca_zoo/_utils/_linalg.py:67-71) and, in Cholesky form, the whitening of _linalg.py:30-38:
- * with R_i = (1-c) C_ii + c I = L_i L_i^T,  T = L_1^-1 C_12 L_2^-T and weights_i = L_i^-T U_k. */
-int ccab_potrf(int dtype, int n, void* A, int64_t lda, double pivot_tol, int* info_dev, void* stream);
-int ccab_trsm(int dtype, int side, int trans, int n, int m, const void* L, int64_t ldl, void* B, int64_t ldb,
-              void* stream);
-
-/* Batched blocked Cholesky WITH the explicit inverse of the factor (the GEMM-friendly form of the whitening):
+ * Batched blocked Cholesky WITH the explicit inverse of the factor (the GEMM-friendly form of the whitening):
  * for each of `batch` SPD matrices A_b = A + b * stride_a (n x n row-major, lower triangle referenced)
  *   lower triangle of A_b <- L_b,   Linv_b = Linv + b * stride_i (n x n, ldi) <- L_b^-1 (zeros above the diagonal).
- * info_dev[b] (device int[batch]) = 0 or the 1-based index of the first pivot <= pivot_tol.
+ * info_dev[b] (device int[batch]) = 0 or the 1-based index of the first pivot <= pivot_tol (matrix not numerically
+ * positive definite: callers fall back to the eigen route).
  * Diagonal blocks (128 wide for float, 64 for double) are factored AND inverted by one single-CTA launch each
  * (warp-synchronous 32 x 32 sub-blocks); panels, trailing updates and the assembly of L^-1 by recursive doubling are
  * GEMMs (wgmma for float).  With Linv,  T = L1^-1 C12 L2^-T  and the weights  L_i^-T U_k  are plain products.
@@ -293,12 +282,6 @@ int ccab_frobenius_norm(int dtype, int m, int n, const void* A, int64_t lda, voi
  * last pair and returns the kernel's duration in ms (-1 if none). */
 int ccab_profile_moments(int enable);
 double ccab_profile_moments_last_ms(void);
-
-/* Debug/tuning knobs ("lbo_bytes", "sbo_bytes", "tma_dtype", "force_splits", "tc_variant", "tc_kc", "x3_split",
- * "x3b_oneshot" = 1: one (tile, split) unit per CTA pair instead of the persistent moment kernel, "f64_simt",
- * "gemm_force_fma", "gemm_split" = 0: never split thin float32 products over k, "jacobi_inner_sweeps",
- * "jacobi_force_unfused"); value < 0 restores the default.  Not part of the stable surface. */
-int ccab_debug_set(const char* key, int value);
 
 #ifdef __cplusplus
 }

@@ -6,7 +6,8 @@ test.  The product keeps failing loudly without a CUDA device (tests/test_abi_cp
 
 Contracts mirrored (see cca_zoo_b200/ops.py and include/ccab200.h): the padded moment buffer ``[Dp*Dp + Dp]`` with
 every view padded to 128-column blocks, eigenvalues descending with eigenvectors as ROWS, ``gesvj`` taking the
-transposed matrix, in-place ``potrf_`` / ``trsm_`` / ``center_columns_`` and their device-side status flags.
+transposed matrix, in-place ``potrf_inv_`` / ``center_columns_`` and the Cholesky status flags (1-based index of the
+first pivot <= pivot_tol).
 """
 from __future__ import annotations
 
@@ -114,35 +115,6 @@ def whiten_rows(lam, Vt, c, floor_add=0.0, floor_dev=None, scale=1.0, rank_tol=0
     return Wt, g.to(Vt.dtype), keep.sum().to(torch.int32).reshape(1)
 
 
-def potrf_(A, pivot_tol=0.0):
-    n = A.shape[0]
-    sym = torch.tril(A) + torch.tril(A, -1).T
-    L, info = torch.linalg.cholesky_ex(sym.to(torch.float64))
-    flag = int(info.item())
-    if flag == 0 and pivot_tol > 0.0:
-        small = (L.diagonal() ** 2 <= pivot_tol).nonzero()
-        flag = int(small[0].item()) + 1 if small.numel() else 0
-    if flag == 0:
-        idx = torch.tril_indices(n, n)
-        A[idx[0], idx[1]] = L[idx[0], idx[1]].to(A.dtype)
-    return torch.tensor([flag], dtype=torch.int32)
-
-
-def trsm_(L, B, side="left", trans=False):
-    Lt = torch.tril(L).to(torch.float64)
-    b64 = B.to(torch.float64)
-    if side == "left":
-        if B.shape[0] != L.shape[0]:
-            raise ValueError("shape mismatch")
-        sol = torch.linalg.solve_triangular(Lt.T if trans else Lt, b64, upper=bool(trans))
-    else:
-        if B.shape[1] != L.shape[0] or not trans:
-            raise ValueError("right side supports B <- B L^-T only")
-        sol = torch.linalg.solve_triangular(Lt, b64.T, upper=False).T      # B L^-T = (L^-1 B^T)^T
-    B.copy_(sol.to(B.dtype))
-    return B
-
-
 def scale(A, rows=None, rows_pow=1, cols=None, cols_pow=1, out=None):
     res = A.clone()
     if rows is not None:
@@ -182,14 +154,24 @@ def ccaloss_small(Cm, d1, d2, eps):
 def potrf_inv_(A, pivot_tol=0.0):
     squeeze = A.dim() == 2
     Ab = A.unsqueeze(0) if squeeze else A
+    n = Ab.shape[-1]
+    idx = torch.tril_indices(n, n)
     infos, invs = [], []
-    for b in range(Ab.shape[0]):
-        info = potrf_(Ab[b], pivot_tol)
-        infos.append(info)
-        L = torch.tril(Ab[b]).to(torch.float64)
-        invs.append(torch.linalg.inv(L).to(A.dtype) if int(info) == 0 else torch.zeros_like(Ab[b]))
+    for a in Ab:
+        sym = torch.tril(a) + torch.tril(a, -1).T
+        L, info = torch.linalg.cholesky_ex(sym.to(torch.float64))
+        flag = int(info.item())
+        if flag == 0 and pivot_tol > 0.0:
+            small = (L.diagonal() ** 2 <= pivot_tol).nonzero()
+            flag = int(small[0].item()) + 1 if small.numel() else 0
+        infos.append(flag)
+        if flag == 0:
+            a[idx[0], idx[1]] = L[idx[0], idx[1]].to(A.dtype)
+            invs.append(torch.linalg.inv(torch.tril(a).to(torch.float64)).to(A.dtype))
+        else:
+            invs.append(torch.zeros_like(a))
     Linv = torch.stack(invs)
-    return (Linv[0] if squeeze else Linv), torch.cat(infos)
+    return (Linv[0] if squeeze else Linv), torch.tensor(infos, dtype=torch.int32)
 
 
 def gemm_batched(A, B, transa=False, transb=False, alpha=1.0):
@@ -235,10 +217,6 @@ def ccaloss_bwd(z1, z2, saved, grad_out):
     g1 = (g1 - g1.mean(dim=0, keepdim=True)) * go
     g2 = (g2 - g2.mean(dim=0, keepdim=True)) * go
     return g1.to(z1.dtype), g2.to(z1.dtype)
-
-
-def debug_set(key, value):
-    return None
 
 
 # ---- device-side fit (csrc/fit.cu) stand-in: same result-block layout and status bits, LAPACK arithmetic ----

@@ -14,8 +14,8 @@ def _spd(n, batch, dtype, seed, cond=50.0):
 
 
 @pytest.mark.parametrize("dtype,tol", [(torch.float32, 2e-4), (torch.float64, 1e-11)])
-@pytest.mark.parametrize("n,batch", [(17, 1), (64, 2), (100, 1), (128, 3), (200, 2), (256, 1), (512, 2), (640, 1),
-                                     (1000, 1), (1024, 2)])
+@pytest.mark.parametrize("n,batch", [(5, 1), (17, 1), (64, 2), (100, 1), (128, 3), (200, 2), (256, 1), (300, 1),
+                                     (512, 2), (640, 1), (1000, 1), (1024, 2)])
 def test_potrf_inv_matches_float64(dtype, tol, n, batch):
     from cca_zoo_b200 import ops
 
@@ -34,8 +34,9 @@ def test_potrf_inv_matches_float64(dtype, tol, n, batch):
     assert float((Li.transpose(1, 2) @ Li @ A64 - eye).abs().max()) < 50 * tol
 
 
-def test_potrf_inv_2d_view_inside_a_larger_matrix_and_fma_route():
-    """Diagonal blocks of one covariance matrix as a strided batch (the rCCA use), and the FMA fallback."""
+def test_potrf_inv_2d_view_inside_a_larger_matrix_and_fma_route_for_an_unaligned_row_stride():
+    """Diagonal blocks of one covariance matrix as a strided batch (the rCCA use, tensor-core panels), and the FMA
+    fallback for matrices whose row stride TMA cannot address."""
     from cca_zoo_b200 import ops
 
     C = torch.zeros(512, 512, dtype=torch.float32)
@@ -47,12 +48,11 @@ def test_potrf_inv_2d_view_inside_a_larger_matrix_and_fma_route():
     assert int(info.max().item()) == 0
     ref = torch.linalg.cholesky(A.double())
     assert float((Linv.double().cpu() @ ref - torch.eye(256, dtype=torch.float64)).abs().max()) < 2e-3
-    ops.debug_set("gemm_force_fma", 1)
-    try:
-        Ad = A.cuda().clone()
-        Linv2, info2 = ops.potrf_inv_(Ad)
-    finally:
-        ops.debug_set("gemm_force_fma", 0)
+    # row stride 257 (not a multiple of 4): the panel and trailing-update GEMMs take the FMA kernel
+    buf = torch.zeros(2 * 256 * 257, dtype=torch.float32, device="cuda")
+    Ad = torch.as_strided(buf, (2, 256, 256), (256 * 257, 257, 1))
+    Ad.copy_(A)
+    Linv2, info2 = ops.potrf_inv_(Ad)
     assert int(info2.max().item()) == 0
     assert float((Linv2 - Linv).abs().max() / Linv.abs().max()) < 1e-4
 

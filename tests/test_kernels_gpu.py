@@ -251,43 +251,6 @@ def test_argument_errors_are_loud():
         ops.gemm(torch.zeros(4, 5, device="cuda"), torch.zeros(4, 5, device="cuda"))
 
 
-@pytest.mark.parametrize("dtype,tol", [(torch.float64, 1e-12), (torch.float32, 2e-5)])
-@pytest.mark.parametrize("n", [5, 64, 100, 300])
-def test_potrf_and_trsm(dtype, tol, n):
-    """A = L L^T and the three triangular solves against float64 torch (cca_zoo/_utils/_linalg.py:67-71 route)."""
-    from cca_zoo_b200 import ops
-
-    g = torch.Generator().manual_seed(n)
-    X = torch.randn(2 * n + 3, n, generator=g, dtype=torch.float64)
-    A64 = X.T @ X / (2 * n) + 0.1 * torch.eye(n, dtype=torch.float64)
-    A = A64.to(dtype).cuda()
-    L = A.clone()
-    info = ops.potrf_(L)
-    assert int(info.item()) == 0
-    Lr = torch.tril(L).double().cpu()
-    assert (Lr @ Lr.T - A.double().cpu()).abs().max() < tol * 10
-    B64 = torch.randn(n, 37, generator=g, dtype=torch.float64)
-    for trans in (False, True):
-        Bs = B64.to(dtype).cuda()
-        ops.trsm_(L, Bs, side="left", trans=trans)
-        ref = torch.linalg.solve_triangular(Lr.T if trans else Lr, B64, upper=trans)
-        assert (Bs.double().cpu() - ref).abs().max() < tol * 200 * ref.abs().max()
-    Br = torch.randn(45, n, generator=g, dtype=torch.float64)
-    Bs = Br.to(dtype).cuda()
-    ops.trsm_(L, Bs, side="right", trans=True)
-    ref = torch.linalg.solve_triangular(Lr, Br.T, upper=False).T
-    assert (Bs.double().cpu() - ref).abs().max() < tol * 200 * ref.abs().max()
-
-
-def test_potrf_flags_indefinite_matrix():
-    from cca_zoo_b200 import ops
-
-    A = torch.eye(80, dtype=torch.float64)
-    A[70, 70] = -1.0
-    info = ops.potrf_(A.cuda())
-    assert int(info.item()) == 71
-
-
 def test_topk_svd_matches_full_svd():
     from cca_zoo_b200 import _solvers
 
