@@ -541,7 +541,10 @@ __global__ void jacobi_init_kernel(const T* __restrict__ in, int64_t ld_in, int6
   if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) c.stat[b] = 0u;
 }
 
-// null2[b] = (10 n eps)^2 ||G_b||_F^2 (one block per matrix, fixed-order reduction: deterministic)
+// null2[b] = (n eps)^2 ||G_b||_F^2 (one block per matrix, fixed-order reduction: deterministic).  n eps ||A||_F bounds the
+// rounding error of a column of A V (|fl(A v) - A v| <= n eps |A| |v|), so a column below it carries no direction.  A
+// larger floor stops refining genuine columns: at 10 n eps ||A||_F, a float32 n = 2700 SPD matrix with eigenvalues in
+// [0.01, 1] had every eigenvalue below 0.048 left unrefined (eigenvalue errors of 7.6e-3).
 template <typename T>
 __global__ void jacobi_scale_kernel(const JacobiCtx<T> c, int n, float* __restrict__ null2) {
   __shared__ double red[32];
@@ -560,7 +563,7 @@ __global__ void jacobi_scale_kernel(const JacobiCtx<T> c, int n, float* __restri
     double t = 0.0;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
     const double ne = (double)n * (double)Eps<T>::v;
-    null2[b] = (float)fmin(100.0 * ne * ne * t, 3.0e38);   // norm threshold 10 n eps ||G||_F
+    null2[b] = (float)fmin(ne * ne * t, 3.0e38);   // norm threshold n eps ||G||_F
   }
 }
 
@@ -749,7 +752,10 @@ int jacobi_solve(const JacobiArgs<T>& a, void* ws, size_t ws_bytes, cudaStream_t
     CCAB_CUDA(cudaGetLastError());
   }
   const T tol = a.tol > 0 ? (T)a.tol : (T)(4.0 * (double)Eps<T>::v * std::sqrt((double)m));
-  const int max_sweeps = a.max_sweeps > 0 ? a.max_sweeps : (std::is_same<T, float>::value ? 16 : 24);
+  // the same cap for both precisions: the block sweeps spend a phase that grows with n before the quadratic one sets in
+  // (a float32 n = 2700 SPD matrix with eigenvalues spread over [0.01, 1] converges in its 17th sweep, to eigenvalue
+  // errors of 0.005 n eps ||A||), and the cap only costs time on a solve that would otherwise be reported unconverged
+  const int max_sweeps = a.max_sweeps > 0 ? a.max_sweeps : 24;
   // fused cluster path: smallest cluster (<= 8 CTAs) whose row slice fits comfortably in shared memory; when none
   // fits (large m), each round runs as three kernels (gram / solve / apply)
   int cs = 0, rows_g = 0, rows_v = 0;
