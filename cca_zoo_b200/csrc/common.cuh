@@ -113,11 +113,20 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 // retires all but the most recently committed group
 __device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// retires all but the N most recently committed groups
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving reads of the accumulators above the wait that retires the MMAs writing them
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(float* d) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// keeps the compiler from moving the writes of A fragment registers below the wgmma_fence that precedes their MMAs
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(uint32_t* a) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(a[i])::"memory");
 }
 
 // Shared-memory matrix descriptor of a K-major tile with 128-byte swizzle: one 128-byte row (32 fp32 reduction
@@ -153,6 +162,22 @@ __device__ __forceinline__ void wgmma_tf32<128>(float* d, uint64_t desc_a, uint6
       : "l"(desc_a), "l"(desc_b), "r"(1));
 }
 
+// d += A (64 x 8, from registers) * B (N x 8, K-major shared)^T in TF32.  A fragment of a thread, in the layout of
+// mma.m16n8k8 tf32 with rows offset by 16*(warp % 4): a[0] (row lane/4, k lane%4), a[1] (row + 8), a[2] (k + 4),
+// a[3] (row + 8, k + 4).  The registers of a must stay unchanged until a wait_group retires the MMA.
+template <int N>
+__device__ __forceinline__ void wgmma_tf32_ra(float* d, const uint32_t* a, uint64_t desc_b);
+
+template <>
+__device__ __forceinline__ void wgmma_tf32_ra<128>(float* d, const uint32_t* a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+}
+
 // 3xTF32 split: hi = x with the low 13 mantissa bits cleared (what the tensor core reads of an fp32 operand),
 // lo = rna_tf32(x - hi) carries the next 11 bits (x = hi + lo + O(2^-21 |x|)).
 __device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float(__float_as_uint(v) & 0xFFFFE000u); }
@@ -163,7 +188,8 @@ __device__ __forceinline__ float tf32_residual(float v) {
 }
 
 // Byte offset of the 16-byte chunk holding reduction indices 4*kg .. 4*kg+3 of row `row` in a K-major tile with
-// 128-byte swizzle (see wgmma_desc_k128).
+// 128-byte swizzle (see wgmma_desc_k128).  The same placement as a TMA box of 128-byte rows loaded with
+// CU_TENSOR_MAP_SWIZZLE_128B into a 1024-byte aligned buffer: there `row` is the box row and kg its 16-byte chunk.
 __device__ __forceinline__ uint32_t k128_offset(int row, int kg) {
   return (uint32_t)row * 128u + ((uint32_t)(kg ^ (row & 7)) << 4);
 }

@@ -70,20 +70,25 @@ float moments_profile_last_ms() {
 // =============================================================================================
 // One CTA = one 128 x 128 tile (A block bi, B block bj >= bi) of M over one split of the sample axis, taken in 32-sample
 // slices by four warpgroups that meet only on mbarriers:
-//   * thread 0 issues the TMA loads of the raw row-major [32 samples x 128 columns] box of each column block into a
-//     ring of raw stages (a diagonal tile loads only A).  Rows past n_rows and columns past the view's width arrive
-//     as zeros;
-//   * warpgroups 0 and 1 transpose each raw stage into the K-major, 128-byte-swizzled operand tiles wgmma reads (the
-//     sample index is the strided one of row-major X, and wgmma reads TF32 only K-major): hi, and in 3xTF32 mode lo,
-//     in a ring of operand stages.  Thread (h, m) owns column m and the 4-sample groups of parity h.  Diagonal tiles
-//     also take the exact fp32 column sums here;
-//   * warpgroups 2 and 3 each run the wgmmas of 64 rows of the tile, one slice of MMAs in flight while the next slice
-//     is transposed.  The 3xTF32 mode issues lo*hi + hi*lo + hi*hi per k-step.
-// The mainloop is bound by shared-memory traffic, about 272 KB per 3xTF32 slice of an off-diagonal tile: 32 KB of TMA
-// writes, 32 KB of transpose reads, 64 KB of hi / lo stores and 144 KB of wgmma operand reads.  A second transpose
-// warpgroup hides the latency of the transpose; deeper rings do not help.
+//   * thread 0 issues the TMA loads of the raw row-major [32 samples x 128 columns] slice of each column block, as
+//     four [32 x 32] boxes with 128-byte swizzle, into a ring of raw stages (a diagonal tile loads only A).  Rows past
+//     n_rows and columns past the view's width arrive as zeros;
+//   * warpgroups 0 and 1 transpose the B block of each raw stage into the K-major, 128-byte-swizzled operand tiles
+//     wgmma reads from shared memory (the sample index is the strided one of row-major X, and wgmma reads TF32 only
+//     K-major): hi, and in 3xTF32 mode lo, in a ring of operand stages.  Thread (h, m) owns column m and the 4-sample
+//     groups of parity h.  A diagonal tile transposes its one block, which serves as B, and takes the exact fp32
+//     column sums here;
+//   * warpgroups 2 and 3 each run the wgmmas of 64 rows of the tile, three k-steps of MMAs in flight while the
+//     fragments of the next are loaded.  They load their A fragments straight from the raw stage into registers
+//     (registers have no major-ness requirement) and split hi / lo there; the 3xTF32 mode issues lo*hi + hi*lo + hi*hi
+//     per k-step.
+// Per 3xTF32 slice of an off-diagonal tile the mainloop moves about 192 KB through shared memory: 32 KB of TMA writes,
+// 16 KB of transpose reads, 32 KB of hi / lo stores of B, 16 KB of A fragment loads and 96 KB of wgmma B reads.
+// The swizzle makes the raw reads conflict-free for both readers: a transpose warp reads one 128-byte box row, and a
+// fragment load takes samples {0,5,2,7} (then {4,1,6,3}) of a k-step on lanes t = lane % 4 = 0..3, so the 32 lanes
+// hit 32 distinct banks.
 struct WgParams {
-  CUtensorMap map[kMaxViews];   // view v: {width, rows} fp32, row pitch lds[v], box 128 columns x 32 rows
+  CUtensorMap map[kMaxViews];   // view v: {width, rows} fp32, row pitch lds[v], box 32 columns x 32 rows, 128B swizzle
   uint8_t blk_view[kMaxBlocks];
   int blk_col0[kMaxBlocks];
   float* partial;      // [S][Dp][Dp]
@@ -97,20 +102,29 @@ static_assert(sizeof(WgParams) <= 4096, "kernel parameter space");
 constexpr int kWgXpose = 256;              // two transpose warpgroups
 constexpr int kWgThreads = kWgXpose + 256;  // + two MMA warpgroups
 constexpr int kWgKC = 32;                  // samples per slice = one 128-byte K-major row
-constexpr int kWgTile = kBlk * kWgKC * 4;  // bytes of one 128 x 32 fp32 tile (raw box or operand copy)
+constexpr int kWgTile = kBlk * kWgKC * 4;  // bytes of one 128 x 32 fp32 tile (raw column block or operand copy)
+constexpr int kWgBox = 32 * kWgKC * 4;     // bytes of one [32 samples x 32 columns] TMA box
+
+// Byte offset of element (sample k, column m) in the raw slice of a column block: box m / 32, swizzled as TMA stores it
+__device__ __forceinline__ uint32_t raw_offset(int k, int m) {
+  return (uint32_t)(m >> 5) * kWgBox + k128_offset(k, (m & 31) >> 2) + (uint32_t)(m & 3) * 4;
+}
 
 template <bool X3>
 struct WgCfg {
-  static constexpr int kOps = X3 ? 2 : 1;              // hi (+ lo) copy of each operand
-  static constexpr int kOpStage = 2 * kOps * kWgTile;  // A copies, then B copies
-  static constexpr int kRawStage = 2 * kWgTile;        // raw A box, raw B box
+  static constexpr int kOps = X3 ? 2 : 1;          // hi (+ lo) copy of the B operand
+  static constexpr int kOpStage = kOps * kWgTile;
+  static constexpr int kRawStage = 2 * kWgTile;    // raw A block, raw B block
   static constexpr int kOpStages = X3 ? 2 : 3;
-  static constexpr int kRawStages = X3 ? 3 : 4;
+  // a raw stage is held until the MMA warps have loaded its A fragments, up to kOpStages slices after its transpose
+  static constexpr int kRawStages = 5;
   static constexpr int kBarOff = kOpStages * kOpStage + kRawStages * kRawStage;
   static constexpr int kSumOff = kBarOff + 2 * (kOpStages + kRawStages) * 8;       // odd column sums
   static constexpr int kSmem = kSumOff + kBlk * 4 + 1024;   // + alignment slack
 };
 static_assert(WgCfg<true>::kSmem <= 227 * 1024 && WgCfg<false>::kSmem <= 227 * 1024, "shared memory per block");
+static_assert(WgCfg<true>::kRawStages > WgCfg<true>::kOpStages && WgCfg<false>::kRawStages > WgCfg<false>::kOpStages,
+              "the refill of a raw stage must not wait on the MMA warps' current slice");
 
 template <bool X3>
 __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __grid_constant__ WgParams p) {
@@ -138,7 +152,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
   if (threadIdx.x == 0) {
     for (int s = 0; s < NR; ++s) {
       mbar_init(&raw_full[s], 1);
-      mbar_init(&raw_empty[s], kWgXpose);   // every transpose thread
+      mbar_init(&raw_empty[s], kWgXpose + 8);   // every transpose thread and one lane of each MMA warp
     }
     for (int s = 0; s < NO; ++s) {
       mbar_init(&op_full[s], kWgXpose);
@@ -158,21 +172,26 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
     auto issue = [&](int c) {
       const int s = c % NR;
       const int row = (int)(p.row_base + r0 + (int64_t)c * kWgKC);
+      uint8_t* dst = raw + s * Cfg::kRawStage;
       mbar_arrive_expect_tx(&raw_full[s], diag ? kWgTile : 2 * kWgTile);
-      tma_load_2d(raw + s * Cfg::kRawStage, mapA, &raw_full[s], colA, row);
-      if (!diag) tma_load_2d(raw + s * Cfg::kRawStage + kWgTile, mapB, &raw_full[s], colB, row);
+#pragma unroll
+      for (int q = 0; q < kBlk / 32; ++q) {
+        tma_load_2d(dst + q * kWgBox, mapA, &raw_full[s], colA + 32 * q, row);
+        if (!diag) tma_load_2d(dst + kWgTile + q * kWgBox, mapB, &raw_full[s], colB + 32 * q, row);
+      }
     };
     if (threadIdx.x == 0)
       for (int c = 0; c < min(NR, nch); ++c) issue(c);
 
     float csum = 0.f;   // column m of a diagonal tile over the 4-sample groups of parity h
-    auto transpose = [&](const float* src, uint8_t* hi, uint8_t* lo, bool sums) {
+    auto transpose = [&](const uint8_t* src, uint8_t* hi, uint8_t* lo, bool sums) {
 #pragma unroll
       for (int j = 0; j < kWgKC / 8; ++j) {
         const int kg = 2 * j + h;
         float v[4];
 #pragma unroll
-        for (int e = 0; e < 4; ++e) v[e] = src[(4 * kg + e) * kBlk + m];   // lanes walk columns: conflict-free
+        for (int e = 0; e < 4; ++e)   // a warp reads one 128-byte box row: conflict-free
+          v[e] = *reinterpret_cast<const float*>(src + raw_offset(4 * kg + e, m));
         const uint32_t off = k128_offset(m, kg);
         *reinterpret_cast<float4*>(hi + off) = make_float4(tf32_hi(v[0]), tf32_hi(v[1]), tf32_hi(v[2]), tf32_hi(v[3]));
         if (X3)
@@ -185,16 +204,17 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
       const int sr = c % NR, so = c % NO;
       mbar_wait(&raw_full[sr], (c / NR) & 1);
       mbar_wait(&op_empty[so], ((c / NO) & 1) ^ 1);   // the MMAs of slice c - NO have retired
-      const float* src = reinterpret_cast<const float*>(raw + sr * Cfg::kRawStage);
       uint8_t* dst = ops + so * Cfg::kOpStage;
-      transpose(src, dst, dst + kWgTile, diag);
-      if (!diag) transpose(src + kBlk * kWgKC, dst + Cfg::kOps * kWgTile, dst + (Cfg::kOps + 1) * kWgTile, false);
+      transpose(raw + sr * Cfg::kRawStage + (diag ? 0 : kWgTile), dst, dst + kWgTile, diag);
       fence_proxy_async_smem();   // the generic-proxy stores become visible to wgmma (async proxy)
       mbar_arrive(&raw_empty[sr]);
       mbar_arrive(&op_full[so]);
-      if (threadIdx.x == 0 && c + NR < nch) {
-        mbar_wait(&raw_empty[sr], (c / NR) & 1);
-        issue(c + NR);
+      // Refill the raw stage of slice c - NO + 1: the MMA warps hand back slice c - NO (seen above) as they load the
+      // last A fragments of slice c - NO + 1, so this wait is short and does not hold the transpose back behind them.
+      const int rf = c + NR - NO + 1;
+      if (threadIdx.x == 0 && rf >= NR && rf < nch) {
+        mbar_wait(&raw_empty[rf % NR], (rf / NR - 1) & 1);
+        issue(rf);
       }
     }
     if (diag) {   // even + odd groups
@@ -206,37 +226,69 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
   } else {
     // ---- MMA warpgroups ----
     setmaxnreg_inc<168>();
-    const int wg = (threadIdx.x - kWgXpose) >> 7;
+    const int wg = (threadIdx.x - kWgXpose) >> 7, lane = threadIdx.x & 31, t = lane & 3;
+    // Raw-stage offsets of this thread's A fragment elements in k-step 0 (k-step kk adds kk * 1024): rows m and m + 8
+    // of the tile, and the two samples of lane t, t and t + 4.  The first load takes sample kx, the second kx ^ 4, so
+    // that the lanes of one load hit distinct swizzle chunks; odd t gets its samples in the swapped order.
+    const int m = wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+    const int kx = t ^ ((t & 1) << 2);
+    const bool swap = t & 1;
+    const uint32_t o00 = raw_offset(kx, m), o01 = raw_offset(kx ^ 4, m);
+    const uint32_t o10 = raw_offset(kx, m + 8), o11 = raw_offset(kx ^ 4, m + 8);
     float acc[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     wgmma_fence_regs<64>(acc);   // keeps the zeroing out of the wgmma pipeline (else ptxas serialises the wgmmas)
+    // One wgmma group per k-step, so that the fragment registers of a k-step are free once its group of the previous
+    // slice has retired: a ring of four k-step fragments, 32 registers in 3xTF32 mode, with three groups in flight
+    // while the next fragments are loaded.  (Two whole-slice fragment sets do not fit next to the accumulators in the
+    // 128 registers a 512-thread CTA compiles to.)
+    constexpr int KS = kWgKC / 8;
+    uint32_t fa[KS][Cfg::kOps][4] = {};   // [k-step][hi, lo][a0..a3]
     for (int c = 0; c < nch; ++c) {
-      const int so = c % NO;
-      mbar_wait(&op_full[so], (c / NO) & 1);
-      const uint32_t st = smem_u32(ops + so * Cfg::kOpStage);
-      const uint32_t a0 = st + wg * 64 * 128;                       // this warpgroup's 64 rows of the A tile
-      const uint32_t b0 = diag ? st : st + Cfg::kOps * kWgTile;     // a diagonal tile multiplies A by itself
-      wgmma_fence();
+      const int sr = c % NR, so = c % NO;
+      mbar_wait(&raw_full[sr], (c / NR) & 1);
+      const uint8_t* a_src = raw + sr * Cfg::kRawStage;   // the A block (a diagonal tile's only block)
+      const uint32_t b0 = smem_u32(ops + so * Cfg::kOpStage);
 #pragma unroll
-      for (int kk = 0; kk < kWgKC / 8; ++kk) {
-        const uint64_t a_hi = wgmma_desc_k128(a0 + 32 * kk), b_hi = wgmma_desc_k128(b0 + 32 * kk);
-        if (X3) {
-          const uint64_t a_lo = wgmma_desc_k128(a0 + kWgTile + 32 * kk), b_lo = wgmma_desc_k128(b0 + kWgTile + 32 * kk);
-          wgmma_tf32<128>(acc, a_lo, b_hi);   // small cross terms first
-          wgmma_tf32<128>(acc, a_hi, b_lo);
+      for (int kk = 0; kk < KS; ++kk) {
+        wgmma_wait<KS - 1>();   // k-step kk of slice c - 1 has retired: its fragment registers may be rewritten
+        // ... and not before: keeping them live up to here makes ptxas give each k-step registers of its own (else it
+        // may reuse one set and serialise the wgmmas)
+        wgmma_fence_regs<Cfg::kOps * 4>(&fa[kk][0][0]);
+        // the last k-step of slice c - 1 has retired with it: hand that slice's operand stage back
+        if (kk == KS - 1 && c > 0 && lane == 0) mbar_arrive(&op_empty[(c - 1) % NO]);
+        const uint8_t* s = a_src + kk * 1024;
+        const float v00 = *reinterpret_cast<const float*>(s + o00), v01 = *reinterpret_cast<const float*>(s + o01);
+        const float v10 = *reinterpret_cast<const float*>(s + o10), v11 = *reinterpret_cast<const float*>(s + o11);
+        const float a[4] = {swap ? v01 : v00, swap ? v11 : v10, swap ? v00 : v01, swap ? v10 : v11};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          fa[kk][0][i] = __float_as_uint(tf32_hi(a[i]));
+          if constexpr (X3) fa[kk][1][i] = __float_as_uint(tf32_residual(a[i]));
         }
-        wgmma_tf32<128>(acc, a_hi, b_hi);
+        wgmma_fence_regs<Cfg::kOps * 4>(&fa[kk][0][0]);
+        if (kk == KS - 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&raw_empty[sr]);   // every lane of the warp has read the slice's A fragments
+        }
+        if (kk == 0) mbar_wait(&op_full[so], (c / NO) & 1);
+        const uint64_t b_hi = wgmma_desc_k128(b0 + 32 * kk);
+        wgmma_fence();
+        if constexpr (X3) {
+          const uint64_t b_lo = wgmma_desc_k128(b0 + kWgTile + 32 * kk);
+          wgmma_tf32_ra<128>(acc, fa[kk][1], b_hi);   // small cross terms first
+          wgmma_tf32_ra<128>(acc, fa[kk][0], b_lo);
+        }
+        wgmma_tf32_ra<128>(acc, fa[kk][0], b_hi);
+        wgmma_commit();
       }
-      wgmma_commit();
-      wgmma_wait_1();   // the MMAs of slice c - 1 have retired: hand their operand stage back
-      if (c > 0 && (threadIdx.x & 31) == 0) mbar_arrive(&op_empty[(c - 1) % NO]);
     }
     wgmma_wait_all();
     wgmma_fence_regs<64>(acc);
 
     // ---- epilogue: fragments -> partial slab of this split ----
-    const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const int warp = (threadIdx.x >> 5) & 3;
     float* P = p.partial + (size_t)split * p.Dp * p.Dp;
     const int row0 = bi * kBlk + wg * 64 + warp * 16 + (lane >> 2);
     const int col0 = bj * kBlk + 2 * (lane & 3);
@@ -620,8 +672,8 @@ EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// Row-major fp32 view (n_rows x d, row pitch ld floats) read in [32 rows x 128 columns] boxes, unswizzled; elements
-// past column d or row n_rows read as zero.
+// Row-major fp32 view (n_rows x d, row pitch ld floats) read in [32 rows x 32 columns] boxes with 128-byte swizzle
+// (see raw_offset); elements past column d or row n_rows read as zero, also in boxes that lie wholly past column d.
 int encode_view_map(CUtensorMap* map, const void* ptr, int64_t n_rows, int64_t d, int64_t ld) {
   EncodeTiledFn enc = encode_fn();
   if (!enc) {
@@ -630,10 +682,10 @@ int encode_view_map(CUtensorMap* map, const void* ptr, int64_t n_rows, int64_t d
   }
   cuuint64_t gdim[2] = {(cuuint64_t)d, (cuuint64_t)n_rows};
   cuuint64_t gstride[1] = {(cuuint64_t)ld * 4};
-  cuuint32_t box[2] = {(cuuint32_t)kBlk, (cuuint32_t)kWgKC};
+  cuuint32_t box[2] = {32, (cuuint32_t)kWgKC};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed with CUresult %d (d=%lld n=%lld ld=%lld)", (int)r, (long long)d,
