@@ -199,6 +199,10 @@ class BaseModel(BaseEstimator, ABC):
         mom.add_(part)
         return mom
 
+    def _solve_dtype(self, in_dtype):
+        """dtype of the covariance and of every solve after it, for views of ``in_dtype``."""
+        return torch.float64 if (self._solve_in_float64 or in_dtype == torch.float64) else torch.float32
+
     def _covariance_stage(self, mom, n_local, dims, in_dtype, check_finite, reduced=False):
         """All-reduce (if sharded and not ``reduced`` already), finalise the covariance, record the fitted metadata
         (_base.py:94-101)."""
@@ -210,7 +214,7 @@ class BaseModel(BaseEstimator, ABC):
         # reference's host scan (check_array) for tensors that never visit the host
         if check_finite and not bool(torch.isfinite(mom).all()):
             raise ValueError("Input contains NaN or infinity.")
-        solve_dtype = torch.float64 if (self._solve_in_float64 or in_dtype == torch.float64) else torch.float32
+        solve_dtype = self._solve_dtype(in_dtype)
         centred = bool(self.center) or self._covariance_always_centred
         C, mean = ops.covariance(mom, dims, n_total, center=centred, dtype=solve_dtype)
         # estimators whose reference mixes np.cov (always centred) with products of the raw views (GCCA, center=False)
@@ -253,7 +257,7 @@ class BaseModel(BaseEstimator, ABC):
             C, dims, n_total = self._covariance_stage(mom, n_local, dims, in_dtype, True)
             return self._finish(self._solve(C, dims, n_total))
         mom, n_host, n_dev = parallel.allreduce_moments_lazy(mom, n_local, dims=dims)
-        solve_dtype = torch.float64 if (self._solve_in_float64 or in_dtype == torch.float64) else torch.float32
+        solve_dtype = self._solve_dtype(in_dtype)
         attempts = plan.pop("iters")
         hdr = None
         for iters in attempts:

@@ -461,7 +461,7 @@ int ccab_potrf_inv(int dtype, int n, int batch, void* A, int64_t lda, int64_t st
 }
 
 size_t ccab_rcca_fit_workspace_bytes(int dtype, const int64_t* dims, int k, int p) {
-  if (!dims || dims[0] < 1 || dims[1] < 1 || k < 1 || p < k) return 0;
+  if (!dims || dims[0] < 1 || dims[1] < 1 || (dtype != CCAB_F32 && dtype != CCAB_F64)) return 0;
   return dtype == CCAB_F32 ? rcca_fit_workspace_bytes<float>((int)dims[0], (int)dims[1], k, p)
                            : rcca_fit_workspace_bytes<double>((int)dims[0], (int)dims[1], k, p);
 }
@@ -549,7 +549,7 @@ int ccab_ccaloss_bwd(int dtype, const void* z1, int64_t ld1, const void* z2, int
 
 size_t ccab_mcca_fit_workspace_bytes(int dtype, int n_views, const int64_t* dims, int k, int p) {
   ColumnLayout L;
-  if (!dims || make_layout(n_views, dims, &L) || k < 1 || p < k) return 0;
+  if (!dims || make_layout(n_views, dims, &L) || (dtype != CCAB_F32 && dtype != CCAB_F64)) return 0;
   return dtype == CCAB_F32 ? mcca_fit_workspace_bytes<float>(L, k, p) : mcca_fit_workspace_bytes<double>(L, k, p);
 }
 

@@ -286,8 +286,10 @@ RccaPlan make_rcca_plan(int d1, int d2, int k, int p) {
 
 }  // namespace
 
+// 0 for every shape rcca_fit refuses: the workspace query is also the question "does the one-call fit take this?"
 template <typename T>
 size_t rcca_fit_workspace_bytes(int d1, int d2, int k, int p) {
+  if (!(k >= 1 && p >= k && p <= std::min(d1, d2) && syevj_small_supported<T>(p))) return 0;
   return make_rcca_plan<T>(d1, d2, k, p).total;
 }
 
@@ -573,8 +575,10 @@ __global__ void copy_vals_kernel(const T* __restrict__ src, T* __restrict__ dst,
 
 }  // namespace
 
+// 0 for every shape mcca_fit refuses (as rcca_fit_workspace_bytes)
 template <typename T>
 size_t mcca_fit_workspace_bytes(const ColumnLayout& L, int k, int p) {
+  if (!(L.n_views >= 2 && k >= 1 && p >= k && p <= L.D && syevj_small_supported<T>(p))) return 0;
   return make_mcca_plan<T>(L, k, p).total;
 }
 

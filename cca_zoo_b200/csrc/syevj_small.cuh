@@ -5,7 +5,7 @@
 namespace ccab {
 
 template <typename T>
-bool syevj_small_supported(int n);   // n <= 128 (float) / ~100 (double): two copies of H and of a column slice of V must fit one CTA's shared memory
+bool syevj_small_supported(int n);   // n <= 128 (float) / 104 (double): two copies of H and of a column slice of V must fit one CTA's shared memory
 
 // For each of `batch` symmetric matrices A_b = A + b * strideA (n x n, lda): eigenvalues descending into
 // evals + b * strideE, eigenvectors as ROWS of evt + b * strideV (n x n, ldv).  info_dev[b] (device, may be NULL) =

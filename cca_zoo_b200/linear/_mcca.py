@@ -7,6 +7,7 @@ from typing import Any, ClassVar
 from sklearn.utils._param_validation import Interval, StrOptions
 
 from .. import ops
+from ..ops import mcca_fit_workspace_bytes   # a host query of the library: needs no device
 from .._base import BaseModel
 from .._solvers import mcca_weights
 from .._validation import perview_parameter, validate_views
@@ -57,7 +58,8 @@ class MCCA(BaseModel):
 
     def _device_fit_plan(self, dims, n_local, in_dtype):
         """Device-side fit (csrc/fit.cu: mcca_fit) for plain MCCA on large, well-posed problems; subclasses that
-        rebuild A / B (GRCCA, PartialCCA) assemble on the host and never get here."""
+        rebuild A / B (GRCCA, PartialCCA) assemble on the host and never get here.  Declined when the library refuses
+        the block width p in the solve dtype (its workspace query answers 0)."""
         if type(self) is not MCCA or self.solver == "eigen":
             return None
         D = int(sum(dims))
@@ -66,7 +68,7 @@ class MCCA(BaseModel):
         k = min(int(self.latent_dimensions), D)
         p = min(D, max(2 * k, k + 32))
         c_ = [float(x) for x in perview_parameter("c", self.c, 0.0, len(dims))]
-        if 4 * k > D or p > 128 or max(c_) > 0.9:
+        if 4 * k > D or max(c_) > 0.9 or mcca_fit_workspace_bytes(dims, k, p, self._solve_dtype(in_dtype)) == 0:
             return None
         eps = float(self.eps)
 

@@ -10,6 +10,7 @@ from sklearn.utils._param_validation import Interval, StrOptions
 
 from .._base import BaseModel
 from .. import ops
+from ..ops import rcca_fit_workspace_bytes   # a host query of the library: needs no device
 from .._solvers import rcca_weights
 from .._validation import perview_parameter, validate_views
 
@@ -72,8 +73,9 @@ class rCCA(BaseModel):
     def _device_fit_plan(self, dims, n_local, in_dtype):
         """The device-side fit (csrc/fit.cu: Cholesky whitening + subspace iteration, everything on the stream) is
         taken for large, well-posed problems: ``solver`` allows it, k is small against the widths (4k <= min d_i) and
-        the iterated block fits the single-CTA Ritz solve (p <= 128).  Whether n > max d_i holds for the TOTAL sample
-        count, and whether the blocks are positive definite, is decided on the device (status word)."""
+        the library takes the iterated block width p in the solve dtype (its workspace query answers 0 otherwise: the
+        single-CTA Ritz solve bounds p).  Whether n > max d_i holds for the TOTAL sample count, and whether the blocks
+        are positive definite, is decided on the device (status word)."""
         if self.solver == "eigen":
             return None
         if self.solver == "auto" and not (min(dims) >= 256 and n_local > max(dims)):
@@ -81,7 +83,7 @@ class rCCA(BaseModel):
         k = min(int(self.latent_dimensions), dims[0], dims[1])
         over = int(os.environ.get("CCAB_FIT_OVERSAMPLE", "0")) or max(16, k // 4)
         p = min(min(dims), k + over)
-        if 4 * k > min(dims) or p > 128:
+        if 4 * k > min(dims) or rcca_fit_workspace_bytes(dims, k, p, self._solve_dtype(in_dtype)) == 0:
             return None
         first = int(os.environ.get("CCAB_FIT_ITERS", "0")) or 6
         c_ = [float(x) for x in perview_parameter("c", self.c, 0.0, 2)]

@@ -272,7 +272,7 @@ def syevj(A: torch.Tensor, shift: float = 0.0, return_info: bool = False):
 
 
 def syevj_small(A: torch.Tensor):
-    """Single-launch eigensolver for small symmetric matrices (n <= 128 float32 / 96 float64), (n,n) or (batch,n,n).
+    """Single-launch eigensolver for small symmetric matrices (n <= 128 float32 / 104 float64), (n,n) or (batch,n,n).
     Returns (evals desc, evecs_t rows, info int32[batch] on the device: sweeps, negative = not converged)."""
     lib = _lib.load()
     _require_cuda(A, "A")
@@ -500,6 +500,16 @@ def potrf_inv_(A, pivot_tol=0.0):
 # status bits of the device-side fit (csrc/fit.cuh)
 FIT_NOT_POSITIVE_DEFINITE, FIT_NOT_CONVERGED, FIT_NON_FINITE, FIT_TOO_FEW_SAMPLES = 1, 2, 4, 8
 FIT_HEADER_DOUBLES = 32
+
+
+def rcca_fit_workspace_bytes(dims, k: int, p: int, dtype) -> int:
+    """Workspace of ``rcca_fit`` in bytes; 0 when the fit refuses this (dims, k, p) in ``dtype``."""
+    return int(_lib.load().ccab_rcca_fit_workspace_bytes(_DT[dtype], _lib.i64_array(dims), int(k), int(p)))
+
+
+def mcca_fit_workspace_bytes(dims, k: int, p: int, dtype) -> int:
+    """Workspace of ``mcca_fit`` in bytes; 0 when the fit refuses this (dims, k, p) in ``dtype``."""
+    return int(_lib.load().ccab_mcca_fit_workspace_bytes(_DT[dtype], len(dims), _lib.i64_array(dims), int(k), int(p)))
 
 
 def rcca_fit(mom: torch.Tensor, dims, n_host, n_dev, center: bool, c, k: int, p: int, iters: int, dtype):

@@ -129,7 +129,7 @@ int ccab_syevj(int dtype, int n, int batch, const void* A, int64_t lda, int64_t 
                void* evals, void* evecs_t, int64_t ldv, int* info, float* info_offdiag, void* workspace,
                size_t workspace_bytes, void* stream);
 
-/* Small symmetric eigenproblems (n <= 128 float / 96 double), batched, ONE single-CTA launch per matrix, no host
+/* Small symmetric eigenproblems (n <= 128 float / 104 double), batched, ONE single-CTA launch per matrix, no host
  * synchronisation: two-sided Jacobi with tournament ordering in shared memory.  Same outputs as ccab_syevj
  * (descending eigenvalues, eigenvectors as rows; evals / evecs_t contiguous per matrix: n and n x ldv); absolute
  * accuracy eps * ||A|| (use ccab_syevj when tiny eigenvalues matter relatively).  info_dev[b] (device int[batch],
@@ -222,7 +222,9 @@ int ccab_potrf_inv(int dtype, int n, int batch, void* A, int64_t lda, int64_t st
  *                 8 too few samples (n <= max d_i);  header[1] = n_total;  [2] residual;  [3] sigma_1;
  *                 [4] index of the first failed factorisation;  [5] sweeps of the Ritz eigensolve
  *   n_total_dev (device double, may be NULL) overrides n_total: the sample count can ride in the all-reduced message.
- *   p must satisfy k <= p <= min(d1, d2, 128).  dtype = arithmetic of the whole solve (CCAB_F32 uses wgmma GEMMs).
+ *   p must satisfy k <= p <= min(d1, d2) and p <= 128 (float) / 104 (double), the sizes ccab_syevj_small takes.
+ *   ccab_rcca_fit_workspace_bytes returns 0 for every (dtype, dims, k, p) the fit refuses, so callers ask it first.
+ *   dtype = arithmetic of the whole solve (CCAB_F32 uses wgmma GEMMs).
  * Replaces cca_zoo/linear/_rcca.py:83-101 (via cca_zoo/_utils/_linalg.py:9-41) after the moment pass. */
 size_t ccab_rcca_fit_workspace_bytes(int dtype, const int64_t* dims, int k, int p);
 int ccab_rcca_fit_result_layout(int dtype, const int64_t* dims, int k, int p, int64_t* offsets /* [5] */);
@@ -237,7 +239,8 @@ int ccab_rcca_fit(int dtype, const int64_t* dims, const double* moments, const d
  * Result block: double header[32] | double mean[D] | T eigenvalues[k] | T W_1[d_1 x k] | .. | T W_m; offsets has m + 3
  * entries (mean, eigenvalues, W_1 .. W_m, total).  `eps` is the reference's floor on lambda_min(B): a block whose pivots
  * fall below it fails the factorisation (status bit 1) and the caller takes the eigen route, which applies the floor.
- * Needs max c <= 0.9 and k <= p <= 128.
+ * Needs max c <= 0.9 and k <= p <= D with p <= 128 (float) / 104 (double); ccab_mcca_fit_workspace_bytes returns 0
+ * for every (dtype, dims, k, p) the fit refuses (also for fewer than 2 views).
  * Replaces cca_zoo/linear/_mcca.py:113-173 (_build_A, _build_B, gevp of cca_zoo/_utils/_linalg.py:44-73). */
 size_t ccab_mcca_fit_workspace_bytes(int dtype, int n_views, const int64_t* dims, int k, int p);
 int ccab_mcca_fit_result_layout(int dtype, int n_views, const int64_t* dims, int k, int p, int64_t* offsets);

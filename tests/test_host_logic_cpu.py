@@ -192,6 +192,32 @@ def test_device_fit_plan_limits(host, monkeypatch):
     monkeypatch.delenv("CCAB_FIT_ITERS")
     assert MCCA(latent_dimensions=32, c=0.1)._device_fit_plan([512] * 4, 125000, f32) is not None
     assert MCCA(latent_dimensions=32, c=0.95)._device_fit_plan([512] * 4, 125000, f32) is None       # shift needs c <= 0.9
+    # the float64 Ritz solve takes p <= 104: the plan asks the library with the SOLVE dtype and declines above it
+    f64 = torch.float64
+    assert rCCA(latent_dimensions=83, c=0.1)._device_fit_plan([400, 400], 5000, f64) is not None     # p = 103
+    assert rCCA(latent_dimensions=84, c=0.1)._device_fit_plan([400, 400], 5000, f64) is None         # p = 105
+    assert rCCA(latent_dimensions=84, c=0.1)._device_fit_plan([400, 400], 5000, f32) is not None     # float32: p <= 128
+    assert rCCA(latent_dimensions=90, c=0.1)._device_fit_plan([400, 400], 5000, f64) is None         # p = 112
+    for dt in (f32, f64):                                 # MCCA solves in float64 whatever the input dtype
+        assert MCCA(latent_dimensions=52)._device_fit_plan([512] * 4, 20000, dt) is not None         # p = 104
+        assert MCCA(latent_dimensions=53)._device_fit_plan([512] * 4, 20000, dt) is None             # p = 106
+        assert MCCA(latent_dimensions=60)._device_fit_plan([512] * 4, 20000, dt) is None             # p = 120
+
+
+def test_fit_workspace_query_answers_zero_exactly_where_the_fit_refuses():
+    """ccab_rcca_fit_workspace_bytes / ccab_mcca_fit_workspace_bytes are the one owner of the fits' limits: the plans
+    ask them (a pure host query, so the real library answers here too, also under the CPU stand-in)."""
+    from cca_zoo_b200 import ops
+
+    for dt, pmax in ((torch.float32, 128), (torch.float64, 104)):
+        for dims, k, p in (([200, 150], 1, 1), ([200, 150], 5, 150), ([200, 150], 5, 151), ([200, 150], 6, 5),
+                           ([200, 150], 0, 4), ([300, 300], 64, pmax), ([300, 300], 64, pmax + 1), ([40, 33], 33, 33)):
+            want = 1 <= k <= p <= min(dims) and p <= pmax
+            assert (ops.rcca_fit_workspace_bytes(dims, k, p, dt) > 0) == want, (dt, dims, k, p)
+        for dims, k, p in (([64, 64], 4, 64), ([65, 1], 4, 66), ([65, 1], 4, 67), ([300] * 8, 8, pmax),
+                           ([300] * 8, 8, pmax + 1), ([300], 4, 8), ([300, 300], 9, 8)):
+            want = len(dims) >= 2 and 1 <= k <= p <= sum(dims) and p <= pmax
+            assert (ops.mcca_fit_workspace_bytes(dims, k, p, dt) > 0) == want, (dt, dims, k, p)
 
 
 def test_cholesky_and_eigen_routes_agree_on_wide_views(host):
