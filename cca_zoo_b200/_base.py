@@ -392,7 +392,7 @@ class BaseModel(BaseEstimator, ABC):
         dims = [int(v.shape[1]) for v in dev_views]
         if dims != list(self.n_features_in_):
             raise ValueError(f"views have {dims} features, the model was fitted on {self.n_features_in_}")
-        mom = ops.moments(dev_views, precision=self.precision)
+        mom, _ = ops.moments_safe(dev_views, precision=self.precision)
         mom, n_total = parallel.allreduce_moments(mom, int(dev_views[0].shape[0]), dims=dims)
         C, _ = ops.covariance(mom, dims, n_total, center=True, dtype=torch.float64)
         off = np.concatenate([[0], np.cumsum(dims)]).astype(int)

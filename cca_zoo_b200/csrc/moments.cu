@@ -348,9 +348,32 @@ __global__ void __launch_bounds__(256) moments_simt_kernel(const SimtParams p) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = T(0);
   T csum[4] = {T(0), T(0), T(0), T(0)};
+  // One accumulator run covers at most kRun rows (as plan_tc bounds the 3xTF32 runs): a fp32 sum over all n rows of a
+  // split would drift by eps * sqrt(n).  Every kRun rows the run is folded into float64 registers and restarts.
+  constexpr int kRun = 2048;
+  double fold[4][4], fold_sum[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    fold_sum[i] = 0.0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) fold[i][j] = 0.0;
+  }
+  auto fold_run = [&]() {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      fold_sum[i] += (double)csum[i];
+      csum[i] = T(0);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        fold[i][j] += (double)acc[i][j];
+        acc[i][j] = T(0);
+      }
+    }
+  };
 
   const int lc = threadIdx.x & 63, lr = threadIdx.x >> 6;  // loader: 4 rows x 64 cols per pass
   for (int64_t r = r0; r < r1; r += KC) {
+    if (r > r0 && (r - r0) % kRun == 0) fold_run();
 #pragma unroll
     for (int i = 0; i < KC / 4; ++i) {
       const int kr = lr + 4 * i;
@@ -376,16 +399,17 @@ __global__ void __launch_bounds__(256) moments_simt_kernel(const SimtParams p) {
     }
     __syncthreads();
   }
+  fold_run();   // a split of at most kRun rows writes its fp32 sums unchanged
   T* P = static_cast<T*>(p.partial) + (size_t)split * p.Dp * p.Dp;
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
     for (int j = 0; j < 4; ++j)
-      P[(size_t)(bi * 64 + ty * 4 + i) * p.Dp + bj * 64 + tx * 4 + j] = acc[i][j];
+      P[(size_t)(bi * 64 + ty * 4 + i) * p.Dp + bj * 64 + tx * 4 + j] = (T)fold[i][j];
   if (bi == bj && ty == 0) {
     T* S = static_cast<T*>(p.partial_sum) + (size_t)split * p.Dp;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) S[bi * 64 + tx * 4 + j] = csum[j];
+    for (int j = 0; j < 4; ++j) S[bi * 64 + tx * 4 + j] = (T)fold_sum[j];
   }
 }
 

@@ -45,8 +45,9 @@ int64_t ccab_launch_count(void);
 /* ---- K1: block moments --------------------------------------------------------------------------
  * M = [X_1 .. X_m]^T [X_1 .. X_m] and s = 1^T [X_1 .. X_m] over the n_rows samples this process
  * holds.  Output `moments` (device, double) has ccab_moments_size() entries: a Dp x Dp padded matrix
- * (each view padded to a multiple of 128 columns; only the upper block triangle is meaningful, the rest
- * is zero) followed by the Dp column sums.  The buffer is additive over row shards: all-reduce(sum) it
+ * (each view padded to a multiple of 128 columns) followed by the Dp column sums.  Entries M[r][c] with r <= c are
+ * the moments; entries below the 128-block diagonal are zero; the strictly lower part (r > c) of a diagonal
+ * 128 x 128 block is unspecified and no consumer reads it.  The buffer is additive over row shards: all-reduce(sum) it
  * across ranks before ccab_covariance.
  * Replaces: np.linalg.svd(X) cca_zoo/_utils/_linalg.py:28, X1_w.T @ X2_w cca_zoo/linear/_rcca.py:96,
  * np.cov(...) cca_zoo/linear/_mcca.py:150-152,166 and cca_zoo/linear/_gcca.py:101,
@@ -84,7 +85,8 @@ int ccab_moments_unshift(int dtype, int n_views, const int64_t* dims, double* mo
  * ccab_moments_pack gathers what the all-reduce has to carry into ONE contiguous float64 message of
  * ccab_moments_packed_size() entries: the upper triangle of 128 x 128 blocks of M (row-major over block pairs),
  * the column sums, the local sample count n and one reserved slot.  Sum it over the ranks (NCCL all-reduce over
- * NVLink), then ccab_moments_unpack restores the moment buffer of ccab_moments (zero below the block diagonal);
+ * NVLink), then ccab_moments_unpack restores the moment buffer of ccab_moments (zero below the block diagonal, the
+ * diagonal blocks copied whole, so their strictly lower parts stay as unspecified as in ccab_moments);
  * packed[size - 2] is the total sample count, which ccab_rcca_fit / ccab_mcca_fit read on the device (n_total_dev). */
 int64_t ccab_moments_packed_size(int n_views, const int64_t* dims);
 int ccab_moments_pack(int n_views, const int64_t* dims, const double* moments, double n_local, double* packed,
