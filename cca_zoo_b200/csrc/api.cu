@@ -7,6 +7,7 @@
 #include <atomic>
 #include <exception>
 
+#include "als.cuh"
 #include "ccaloss.cuh"
 #include "cholinv.cuh"
 #include "common.cuh"
@@ -582,6 +583,37 @@ int ccab_mcca_fit(int dtype, int n_views, const int64_t* dims, const double* mom
                            workspace, workspace_bytes, s);
   return mcca_fit<double>(L, moments, n_total_dev, n_total, center, c, eps, k, p, iters, result, result_bytes, workspace,
                           workspace_bytes, s);
+  CCAB_CATCH
+}
+
+size_t ccab_als_fit_workspace_bytes(int n_views, const int64_t* dims) {
+  ColumnLayout L;
+  if (!dims || n_views < 2 || make_layout(n_views, dims, &L)) return 0;
+  return als_fit_workspace_bytes(L);
+}
+
+int ccab_als_fit(int kind, int n_views, const int64_t* dims, const double* G, double g_scale, double n_samples,
+                 const double* params, double mu, const double* init, int k, int max_iter, double tol, double* W_out,
+                 int* iters_out, void* workspace, size_t workspace_bytes, void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(kind >= CCAB_ALS_PLS && kind <= CCAB_ALS_ADMM, "bad ALS kind %d", kind);
+  CCAB_CHECK_ARG(n_views >= 2, "the ALS estimators need at least 2 views, got %d", n_views);
+  CCAB_CHECK_ARG(dims && G && init && W_out && iters_out && workspace, "null pointer argument");
+  CCAB_CHECK_ARG(kind == CCAB_ALS_PLS || params, "params is NULL");
+  CCAB_CHECK_ARG(k >= 1 && max_iter >= 0, "bad k %d / max_iter %d", k, max_iter);
+  CCAB_CHECK_ARG(kind != CCAB_ALS_ADMM || (mu > 0.0 && n_samples > 0.0), "ADMM needs mu > 0 and n_samples > 0");
+  ColumnLayout L;
+  int rc = make_layout(n_views, dims, &L);
+  if (rc) return rc;
+  for (int v = 0; kind != CCAB_ALS_PLS && v < n_views; ++v) {
+    CCAB_CHECK_ARG(params[v] >= 0.0, "params[%d] = %g is negative", v, params[v]);
+    CCAB_CHECK_ARG(kind != CCAB_ALS_SPAN || (params[v] >= 1.0 && params[v] == (double)(int64_t)params[v]),
+                   "span[%d] = %g is not a positive integer", v, params[v]);
+  }
+  rc = require_device();
+  if (rc) return rc;
+  return als_fit(kind, L, G, g_scale, n_samples, params, mu, init, k, max_iter, tol, W_out, iters_out, workspace,
+                 workspace_bytes, static_cast<cudaStream_t>(stream));
   CCAB_CATCH
 }
 

@@ -4,5 +4,7 @@ from ._mcca import MCCA
 from ._gcca import GCCA
 from ._partialcca import PartialCCA
 from ._grcca import GRCCA
+from ._iterative import PLS_ALS, SCCA_ADMM, SCCA_PMD, ParkhomenkoCCA, SCCA_Span
 
-__all__ = ["CCA", "rCCA", "PLS", "MCCA", "GCCA", "PartialCCA", "GRCCA"]
+__all__ = ["CCA", "rCCA", "PLS", "MCCA", "GCCA", "PartialCCA", "GRCCA", "PLS_ALS", "SCCA_PMD", "ParkhomenkoCCA",
+           "SCCA_Span", "SCCA_ADMM"]

@@ -579,6 +579,36 @@ def decode_fit_block(host: torch.Tensor, offsets, dims, k: int, dtype):
     return hdr, mean, sig, ws
 
 
+ALS_KINDS = {"pls": 0, "pmd": 1, "parkhomenko": 2, "span": 3, "admm": 4}
+
+
+def als_fit(cov, dims, n_total, kind: str, params, init, max_iter: int, tol: float, mu: float = 1.0):
+    """Sparse / ALS fit on the block covariance (ccab_als_fit): ``cov`` is the float64 D x D covariance on the device,
+    the iteration runs on the Gram matrix (n_total - 1) cov.  ``init`` (k x D float64, host or device) holds the
+    initial weights of every dimension.  Returns (W (D x k float64 numpy), sweeps per dimension) after ONE copy to the
+    host."""
+    import numpy as np
+
+    lib = _lib.load()
+    _require_cuda(cov, "cov")
+    if cov.dtype != torch.float64:
+        raise ValueError("als_fit iterates in float64")
+    cov = cov.contiguous()
+    D, k = int(sum(dims)), int(init.shape[0])
+    d = _lib.i64_array(dims)
+    init = torch.as_tensor(init, dtype=torch.float64).to(cov.device).contiguous()
+    out = torch.empty(D * k + (k + 1) // 2, dtype=torch.float64, device=cov.device)   # W | int32 sweeps[k]
+    ws = _ws(lib.ccab_als_fit_workspace_bytes(len(dims), d), cov.device)
+    pp = (C.c_double * len(dims))(*[float(x) for x in params])
+    with torch.cuda.device(cov.device):
+        rc = lib.ccab_als_fit(ALS_KINDS[kind], len(dims), d, _ptr(cov), float(n_total - 1), float(n_total), pp,
+                              float(mu), _ptr(init), k, int(max_iter), float(tol), _ptr(out),
+                              C.c_void_p(out.data_ptr() + 8 * D * k), _ptr(ws), ws.numel(), _stream(cov))
+    _lib.check(rc, "ccab_als_fit")
+    host = out.cpu().numpy()
+    return host[:D * k].reshape(D, k).copy(), host[D * k:].view(np.int32)[:k].astype(int).tolist()
+
+
 _POW = {None: 0, 1: 0, -1: 1, -0.5: 2}
 
 

@@ -250,6 +250,32 @@ int ccab_mcca_fit(int dtype, int n_views, const int64_t* dims, const double* mom
                   double n_total, int center, const double* c, double eps, int k, int p, int iters, void* result,
                   size_t result_bytes, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- the sparse / ALS estimators behind the ABI ----------------------------------------------------------------------
+ * PLS_ALS, SCCA_PMD, ParkhomenkoCCA, SCCA_Span and SCCA_ADMM iterated on the block Gram matrix g_scale * G (D x D,
+ * device, row-major, symmetric; pass the covariance with g_scale = n - 1) instead of the samples, all k latent
+ * dimensions in ONE asynchronous call: per dimension one persistent cooperative kernel (every sweep, every view update,
+ * the thresholding and the convergence test: max_i ||w_i - w_i_prev|| < tol, at most max_iter sweeps), then the
+ * deflation X_i <- X_i (I - w_i a_i^T / s_i) as a rank-2m update of a workspace copy of G.  Fixed-order reductions
+ * only: repeated calls give bit-identical results.
+ *   kind       CCAB_ALS_*
+ *   params     per-view (host, n_views doubles): PMD tau (L1 bound tau * sqrt(d_i)), Parkhomenko / ADMM tau, Span span
+ *              (1 <= span); ignored (may be NULL) for PLS_ALS
+ *   mu         ADMM penalty; n_samples: the ADMM step 1 / (||G_ii||_F / n_samples + mu)
+ *   init       device, k x D: the initial weights of each dimension (unit norm per view)
+ *   W_out      device, D x k row-major (hstack of the views' weights);  iters_out: device int[k], sweeps per dimension
+ * Needs 2 <= n_views <= 8; the widest view must fit the shared memory of one CTA (up to ~28000 features).
+ * Replaces cca_zoo/linear/_iterative.py:65-117 (fit / _fit_single with the _update_weight of each model) and
+ * deflate (cca_zoo/_utils/_linalg.py:91-116). */
+#define CCAB_ALS_PLS 0
+#define CCAB_ALS_PMD 1
+#define CCAB_ALS_PARKHOMENKO 2
+#define CCAB_ALS_SPAN 3
+#define CCAB_ALS_ADMM 4
+size_t ccab_als_fit_workspace_bytes(int n_views, const int64_t* dims);
+int ccab_als_fit(int kind, int n_views, const int64_t* dims, const double* G, double g_scale, double n_samples,
+                 const double* params, double mu, const double* init, int k, int max_iter, double tol, double* W_out,
+                 int* iters_out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- the deep-CCA objective behind the ABI (any widths) ---------------------------------------------------------
  * ccab_ccaloss_fwd: loss[0] = -|| S11^-1/2 S12 S22^-1/2 ||_F^2 with S_ii = cov(z_i) + eps I, from the moment pass over
  * [z1 z2] (precision as in ccab_moments), a batched Cholesky + inverse and 7 GEMMs; `saved`
