@@ -3,7 +3,8 @@
 //   * moments_wgmma_kernel : Hopper wgmma (TF32, fp32 accumulators in registers), 128 x 128 tiles of the upper
 //     block triangle, split over the sample axis.  A producer / consumer pipeline on mbarriers: TMA loads of the raw
 //     sample slices, two transpose warpgroups that write them as K-major swizzled shared tiles, two wgmma
-//     warpgroups.  Optional 3xTF32 (hi / lo copies in shared memory, 3 MMAs per k-step) for fp32-grade accuracy.
+//     warpgroups.  Optional 3xTF32 (hi / lo copies in shared memory, 3 MMAs per k-step) for fp32-grade accuracy,
+//     with the two cross terms either in TF32 or as bf16 MMAs (2 instead of 3 units of tensor work).
 //     Column sums are exact fp32 sums of the loaded values.
 //   * moments_simt_kernel : exact FMA (fp32) tile kernel, the non-tensor reference path;
 //     moments_dmma_kernel : float64 inputs on the fp64 tensor pipe (mma.sync m8n8k4.f64).
@@ -87,6 +88,18 @@ float moments_profile_last_ms() {
 // The swizzle makes the raw reads conflict-free for both readers: a transpose warp reads one 128-byte box row, and a
 // fragment load takes samples {0,5,2,7} (then {4,1,6,3}) of a k-step on lanes t = lane % 4 = 0..3, so the 32 lanes
 // hit 32 distinct banks.
+//
+// X3B mode (3xTF32 with bf16 cross terms): hi*hi stays a TF32 MMA per k-step of 8 samples, and lo*hi + hi*lo run as
+// bf16 m64n128k16 MMAs per k16 step of 16 samples, at twice the TF32 rate.  hi = trunc_tf32(x); the bf16 copies are
+// rne_bf16(hi) and rne_bf16(x - hi).  A bf16 k16 step takes its k index in the order of the registers an MMA thread
+// already holds for two TF32 k-steps: logical k 2t, 2t+1, 2t+8, 2t+9 of the step are samples t, t+4, 8+t, 12+t.  (Any
+// sample permutation leaves X^T X unchanged as long as A and B share it.)  So the bf16 A fragment is packed from the
+// TF32 fragment's registers, and chunk e (16 bytes) of a row of the bf16 B tile holds the pairs (8e+t, 8e+t+4),
+// t = 0..3.  The bf16 tile is one 128 x 128-byte K-major tile with 128-byte swizzle: hi in bytes 0..63 of a row (k16
+// steps 0, 1), lo in bytes 64..127.  An operand stage is the TF32 hi tile and this tile, 32 KB as in X3.  The two
+// samples of a pair belong to different parity groups, so an X3B transpose thread (h, m) owns the k16 step h.
+// Per slice of an off-diagonal tile that is 8 TF32 + 8 bf16 MMAs (the tensor time of 16 TF32 MMAs, 24 in X3) and about
+// 160 KB of shared-memory traffic: 32 KB TMA, 16 KB transpose reads, 32 KB stores, 16 KB A fragments, 64 KB B reads.
 struct WgParams {
   CUtensorMap map[kMaxViews];   // view v: {width, rows} fp32, row pitch lds[v], box 32 columns x 32 rows, 128B swizzle
   uint8_t blk_view[kMaxBlocks];
@@ -110,25 +123,32 @@ __device__ __forceinline__ uint32_t raw_offset(int k, int m) {
   return (uint32_t)(m >> 5) * kWgBox + k128_offset(k, (m & 31) >> 2) + (uint32_t)(m & 3) * 4;
 }
 
-template <bool X3>
+// Operand arithmetic of the kernel: one TF32 pass, 3xTF32, 3xTF32 with the cross terms as bf16 MMAs
+enum class K1Mode { TF32, X3, X3B };
+
+template <K1Mode M>
 struct WgCfg {
-  static constexpr int kOps = X3 ? 2 : 1;          // hi (+ lo) copy of the B operand
+  static constexpr int kOps = M == K1Mode::TF32 ? 1 : 2;   // B operand tiles: hi (+ lo, or + bf16 hi | lo)
   static constexpr int kOpStage = kOps * kWgTile;
   static constexpr int kRawStage = 2 * kWgTile;    // raw A block, raw B block
-  static constexpr int kOpStages = X3 ? 2 : 3;
+  static constexpr int kOpStages = M == K1Mode::TF32 ? 3 : 2;
   // a raw stage is held until the MMA warps have loaded its A fragments, up to kOpStages slices after its transpose
   static constexpr int kRawStages = 5;
   static constexpr int kBarOff = kOpStages * kOpStage + kRawStages * kRawStage;
   static constexpr int kSumOff = kBarOff + 2 * (kOpStages + kRawStages) * 8;       // odd column sums
   static constexpr int kSmem = kSumOff + kBlk * 4 + 1024;   // + alignment slack
 };
-static_assert(WgCfg<true>::kSmem <= 227 * 1024 && WgCfg<false>::kSmem <= 227 * 1024, "shared memory per block");
-static_assert(WgCfg<true>::kRawStages > WgCfg<true>::kOpStages && WgCfg<false>::kRawStages > WgCfg<false>::kOpStages,
+static_assert(WgCfg<K1Mode::X3>::kSmem <= 227 * 1024 && WgCfg<K1Mode::TF32>::kSmem <= 227 * 1024 &&
+              WgCfg<K1Mode::X3B>::kSmem <= 227 * 1024, "shared memory per block");
+static_assert(WgCfg<K1Mode::X3>::kRawStages > WgCfg<K1Mode::X3>::kOpStages &&
+              WgCfg<K1Mode::TF32>::kRawStages > WgCfg<K1Mode::TF32>::kOpStages &&
+              WgCfg<K1Mode::X3B>::kRawStages > WgCfg<K1Mode::X3B>::kOpStages,
               "the refill of a raw stage must not wait on the MMA warps' current slice");
 
-template <bool X3>
+template <K1Mode M>
 __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __grid_constant__ WgParams p) {
-  using Cfg = WgCfg<X3>;
+  using Cfg = WgCfg<M>;
+  constexpr bool X3 = M == K1Mode::X3;
   constexpr int NO = Cfg::kOpStages, NR = Cfg::kRawStages;
   extern __shared__ uint8_t smem_raw[];
   // offset (not an integer round trip) so that the compiler still sees shared-memory pointers: LDS / STS, not LD / ST
@@ -183,21 +203,43 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
     if (threadIdx.x == 0)
       for (int c = 0; c < min(NR, nch); ++c) issue(c);
 
-    float csum = 0.f;   // column m of a diagonal tile over the 4-sample groups of parity h
+    float csum = 0.f;   // column m of a diagonal tile over the 4-sample groups of parity h (X3B: k16 step h)
     auto transpose = [&](const uint8_t* src, uint8_t* hi, uint8_t* lo, bool sums) {
+      if constexpr (M == K1Mode::X3B) {   // lo: the bf16 tile, hi | lo pairs of k-step e in chunks e | 4 + e
 #pragma unroll
-      for (int j = 0; j < kWgKC / 8; ++j) {
-        const int kg = 2 * j + h;
-        float v[4];
+        for (int q = 0; q < 2; ++q) {
+          const int e = 2 * h + q;   // k-step of 8 samples
+          float v[8], x[8];
 #pragma unroll
-        for (int e = 0; e < 4; ++e)   // a warp reads one 128-byte box row: conflict-free
-          v[e] = *reinterpret_cast<const float*>(src + raw_offset(4 * kg + e, m));
-        const uint32_t off = k128_offset(m, kg);
-        *reinterpret_cast<float4*>(hi + off) = make_float4(tf32_hi(v[0]), tf32_hi(v[1]), tf32_hi(v[2]), tf32_hi(v[3]));
-        if (X3)
-          *reinterpret_cast<float4*>(lo + off) = make_float4(tf32_residual(v[0]), tf32_residual(v[1]),
-                                                             tf32_residual(v[2]), tf32_residual(v[3]));
-        if (sums) csum += (v[0] + v[1]) + (v[2] + v[3]);
+          for (int i = 0; i < 8; ++i) {   // a warp reads one 128-byte box row: conflict-free
+            v[i] = *reinterpret_cast<const float*>(src + raw_offset(8 * e + i, m));
+            x[i] = tf32_hi(v[i]);
+          }
+          *reinterpret_cast<float4*>(hi + k128_offset(m, 2 * e)) = make_float4(x[0], x[1], x[2], x[3]);
+          *reinterpret_cast<float4*>(hi + k128_offset(m, 2 * e + 1)) = make_float4(x[4], x[5], x[6], x[7]);
+          *reinterpret_cast<uint4*>(lo + k128_offset(m, e)) =
+              make_uint4(pack_bf16x2(x[0], x[4]), pack_bf16x2(x[1], x[5]), pack_bf16x2(x[2], x[6]),
+                         pack_bf16x2(x[3], x[7]));
+          *reinterpret_cast<uint4*>(lo + k128_offset(m, 4 + e)) =
+              make_uint4(pack_bf16x2(v[0] - x[0], v[4] - x[4]), pack_bf16x2(v[1] - x[1], v[5] - x[5]),
+                         pack_bf16x2(v[2] - x[2], v[6] - x[6]), pack_bf16x2(v[3] - x[3], v[7] - x[7]));
+          if (sums) csum += ((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]));
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < kWgKC / 8; ++j) {
+          const int kg = 2 * j + h;
+          float v[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e)   // a warp reads one 128-byte box row: conflict-free
+            v[e] = *reinterpret_cast<const float*>(src + raw_offset(4 * kg + e, m));
+          const uint32_t off = k128_offset(m, kg);
+          *reinterpret_cast<float4*>(hi + off) = make_float4(tf32_hi(v[0]), tf32_hi(v[1]), tf32_hi(v[2]), tf32_hi(v[3]));
+          if (X3)
+            *reinterpret_cast<float4*>(lo + off) = make_float4(tf32_residual(v[0]), tf32_residual(v[1]),
+                                                               tf32_residual(v[2]), tf32_residual(v[3]));
+          if (sums) csum += (v[0] + v[1]) + (v[2] + v[3]);
+        }
       }
     };
     for (int c = 0; c < nch; ++c) {
@@ -239,12 +281,18 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     wgmma_fence_regs<64>(acc);   // keeps the zeroing out of the wgmma pipeline (else ptxas serialises the wgmmas)
-    // One wgmma group per k-step, so that the fragment registers of a k-step are free once its group of the previous
-    // slice has retired: a ring of four k-step fragments, 32 registers in 3xTF32 mode, with three groups in flight
-    // while the next fragments are loaded.  (Two whole-slice fragment sets do not fit next to the accumulators in the
-    // 128 registers a 512-thread CTA compiles to.)
-    constexpr int KS = kWgKC / 8;
-    uint32_t fa[KS][Cfg::kOps][4] = {};   // [k-step][hi, lo][a0..a3]
+    // One wgmma group per step, so that the fragment registers of a step are free once its group of the previous
+    // slice has retired.  A step is one k-step of 8 samples: a ring of four k-step fragments, 32 registers in 3xTF32
+    // mode, with three groups in flight while the next fragments are loaded.  (Two whole-slice fragment sets do not fit
+    // next to the accumulators in the 128 registers a 512-thread CTA compiles to.)  In X3B a step is a k16 step: the
+    // TF32 hi fragments of its two k-steps and the bf16 hi and lo fragments of the k16 MMAs, a ring of two steps (32
+    // registers) with one group in flight.
+    constexpr int KQ = M == K1Mode::X3B ? 2 : 1;                   // k-steps per step
+    constexpr int KS = kWgKC / (8 * KQ);                            // steps per slice
+    constexpr int KR = M == K1Mode::X3B ? 16 : Cfg::kOps * 4;       // fragment registers per step
+    // fragment registers of a step: 0..3 TF32 hi, 4..7 TF32 lo; X3B: 0..3 and 4..7 TF32 hi of its two k-steps,
+    // 8..11 bf16 hi, 12..15 bf16 lo
+    uint32_t fa[KS][KR] = {};
     for (int c = 0; c < nch; ++c) {
       const int sr = c % NR, so = c % NO;
       mbar_wait(&raw_full[sr], (c / NR) & 1);
@@ -252,35 +300,55 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
       const uint32_t b0 = smem_u32(ops + so * Cfg::kOpStage);
 #pragma unroll
       for (int kk = 0; kk < KS; ++kk) {
-        wgmma_wait<KS - 1>();   // k-step kk of slice c - 1 has retired: its fragment registers may be rewritten
-        // ... and not before: keeping them live up to here makes ptxas give each k-step registers of its own (else it
+        wgmma_wait<KS - 1>();   // step kk of slice c - 1 has retired: its fragment registers may be rewritten
+        // ... and not before: keeping them live up to here makes ptxas give each step registers of its own (else it
         // may reuse one set and serialise the wgmmas)
-        wgmma_fence_regs<Cfg::kOps * 4>(&fa[kk][0][0]);
-        // the last k-step of slice c - 1 has retired with it: hand that slice's operand stage back
+        wgmma_fence_regs<KR>(fa[kk]);
+        // the last step of slice c - 1 has retired with it: hand that slice's operand stage back
         if (kk == KS - 1 && c > 0 && lane == 0) mbar_arrive(&op_empty[(c - 1) % NO]);
-        const uint8_t* s = a_src + kk * 1024;
-        const float v00 = *reinterpret_cast<const float*>(s + o00), v01 = *reinterpret_cast<const float*>(s + o01);
-        const float v10 = *reinterpret_cast<const float*>(s + o10), v11 = *reinterpret_cast<const float*>(s + o11);
-        const float a[4] = {swap ? v01 : v00, swap ? v11 : v10, swap ? v00 : v01, swap ? v10 : v11};
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          fa[kk][0][i] = __float_as_uint(tf32_hi(a[i]));
-          if constexpr (X3) fa[kk][1][i] = __float_as_uint(tf32_residual(a[i]));
+        for (int q = 0; q < KQ; ++q) {
+          const uint8_t* s = a_src + (KQ * kk + q) * 1024;
+          const float v00 = *reinterpret_cast<const float*>(s + o00), v01 = *reinterpret_cast<const float*>(s + o01);
+          const float v10 = *reinterpret_cast<const float*>(s + o10), v11 = *reinterpret_cast<const float*>(s + o11);
+          const float a[4] = {swap ? v01 : v00, swap ? v11 : v10, swap ? v00 : v01, swap ? v10 : v11};
+          float x[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            x[i] = tf32_hi(a[i]);
+            fa[kk][4 * q + i] = __float_as_uint(x[i]);
+            if constexpr (X3) fa[kk][4 + i] = __float_as_uint(tf32_residual(a[i]));
+          }
+          if constexpr (M == K1Mode::X3B) {
+            // bf16 register 2q + r: row g + 8r, samples t (low half) and t + 4 of k-step q of the step
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+              fa[kk][8 + 2 * q + r] = pack_bf16x2(x[r], x[r + 2]);
+              fa[kk][12 + 2 * q + r] = pack_bf16x2(a[r] - x[r], a[r + 2] - x[r + 2]);
+            }
+          }
         }
-        wgmma_fence_regs<Cfg::kOps * 4>(&fa[kk][0][0]);
+        wgmma_fence_regs<KR>(fa[kk]);
         if (kk == KS - 1) {
           __syncwarp();
           if (lane == 0) mbar_arrive(&raw_empty[sr]);   // every lane of the warp has read the slice's A fragments
         }
         if (kk == 0) mbar_wait(&op_full[so], (c / NO) & 1);
-        const uint64_t b_hi = wgmma_desc_k128(b0 + 32 * kk);
         wgmma_fence();
-        if constexpr (X3) {
-          const uint64_t b_lo = wgmma_desc_k128(b0 + kWgTile + 32 * kk);
-          wgmma_tf32_ra<128>(acc, fa[kk][1], b_hi);   // small cross terms first
-          wgmma_tf32_ra<128>(acc, fa[kk][0], b_lo);
+        if constexpr (M == K1Mode::X3B) {   // bf16 tile: hi of k16 step kk at 32 kk, lo at 64 + 32 kk
+          wgmma_bf16_ra<128>(acc, &fa[kk][12], wgmma_desc_k128(b0 + kWgTile + 32 * kk));        // lo * hi
+          wgmma_bf16_ra<128>(acc, &fa[kk][8], wgmma_desc_k128(b0 + kWgTile + 64 + 32 * kk));    // hi * lo
+          wgmma_tf32_ra<128>(acc, &fa[kk][0], wgmma_desc_k128(b0 + 64 * kk));
+          wgmma_tf32_ra<128>(acc, &fa[kk][4], wgmma_desc_k128(b0 + 64 * kk + 32));
+        } else {
+          const uint64_t b_hi = wgmma_desc_k128(b0 + 32 * kk);
+          if constexpr (X3) {
+            const uint64_t b_lo = wgmma_desc_k128(b0 + kWgTile + 32 * kk);
+            wgmma_tf32_ra<128>(acc, &fa[kk][4], b_hi);   // small cross terms first
+            wgmma_tf32_ra<128>(acc, &fa[kk][0], b_lo);
+          }
+          wgmma_tf32_ra<128>(acc, &fa[kk][0], b_hi);
         }
-        wgmma_tf32_ra<128>(acc, fa[kk][0], b_hi);
         wgmma_commit();
       }
     }
@@ -608,7 +676,7 @@ struct TcPlan {
 };
 
 TcPlan plan_tc(const ColumnLayout& L, int64_t n_rows, int mode) {
-  const bool x3 = mode != 0;   // 0: one TF32 pass, 1 and 3: 3xTF32
+  const bool x3 = mode != 0;   // 0: one TF32 pass, 1: 3xTF32, 3: 3xTF32 with bf16 cross terms
   TcPlan P;
   P.total_chunks = (int)ceil_div(n_rows, kWgKC);
   P.ntiles = L.nblocks * (L.nblocks + 1) / 2;
@@ -766,6 +834,15 @@ int moments_tf32(const ColumnLayout& L, const void* const* views, const int64_t*
 }
 
 namespace {
+template <K1Mode M>
+int launch_wgmma(dim3 grid, const WgParams& prm, cudaStream_t stream) {
+  // function attributes are per device / context: set on every call
+  CCAB_CUDA(cudaFuncSetAttribute(moments_wgmma_kernel<M>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 WgCfg<M>::kSmem));
+  moments_wgmma_kernel<M><<<grid, kWgThreads, WgCfg<M>::kSmem, stream>>>(prm);
+  return 0;
+}
+
 // One pass over rows [row_base, row_base + n_rows).  Its splits end on multiples of 32 rows from row_base, and a pass
 // that is not the last ends on a multiple of 2048, so no slice reads rows of the next pass.
 int moments_tf32_pass(const ColumnLayout& L, WgParams& prm, int64_t row_base, int64_t n_rows, int mode,
@@ -786,16 +863,10 @@ int moments_tf32_pass(const ColumnLayout& L, WgParams& prm, int64_t row_base, in
   prm.Dp = L.Dp;
   dim3 grid(P.ntiles, P.num_splits);
   if (g_prof_on) cudaEventRecord(g_prof_e0, stream);
-  if (mode != 0) {
-    // function attributes are per device / context: set on every call
-    CCAB_CUDA(cudaFuncSetAttribute(moments_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   WgCfg<true>::kSmem));
-    moments_wgmma_kernel<true><<<grid, kWgThreads, WgCfg<true>::kSmem, stream>>>(prm);
-  } else {
-    CCAB_CUDA(cudaFuncSetAttribute(moments_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   WgCfg<false>::kSmem));
-    moments_wgmma_kernel<false><<<grid, kWgThreads, WgCfg<false>::kSmem, stream>>>(prm);
-  }
+  int rc = mode == 3   ? launch_wgmma<K1Mode::X3B>(grid, prm, stream)
+           : mode != 0 ? launch_wgmma<K1Mode::X3>(grid, prm, stream)
+                       : launch_wgmma<K1Mode::TF32>(grid, prm, stream);
+  if (rc) return rc;
   count_launches(1);
   CCAB_CUDA(cudaGetLastError());
   if (g_prof_on) {

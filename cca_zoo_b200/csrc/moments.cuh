@@ -25,8 +25,8 @@ int make_layout(int n_views, const int64_t* dims, ColumnLayout* out);
 
 // --- launchers (all asynchronous on `stream`) -------------------------------------------------
 // precision: 0 = TF32 single pass (wgmma), 1 = 3xTF32 split (wgmma), 2 = exact SIMT FMA,
-//            3 = 3xTF32 (on Hopper the same kernel as 1; the bf16 cross-term variant needs a TF32 MMA that reads
-//            MN-major operands, which wgmma does not have).
+//            3 = 3xTF32 with the two cross terms as bf16 MMAs (hi*hi in TF32): 2 instead of 3 units of tensor work,
+//            the same split plan and passes as 1.
 size_t moments_workspace_bytes(int dtype, int precision, const ColumnLayout& L, int64_t n_rows);
 
 int moments_tf32(const ColumnLayout& L, const void* const* views, const int64_t* lds, int64_t n_rows,

@@ -33,7 +33,7 @@ extern "C" {
 #define CCAB_PREC_TF32 0   /* fp32 in, one wgmma TF32 pass, fp32 accumulate               */
 #define CCAB_PREC_TF32X3 1 /* fp32 in, hi/lo split + 3 wgmma passes: fp32-grade accuracy          */
 #define CCAB_PREC_EXACT 2  /* FMA in the input dtype on CUDA cores (the only choice for CCAB_F64)  */
-#define CCAB_PREC_TF32X3B 3 /* 3xTF32 with the two cross terms as bf16 MMAs (kind::f16): fp32-grade, 2/3 the tensor work */
+#define CCAB_PREC_TF32X3B 3 /* 3xTF32 with the two cross terms as bf16 MMAs: fp32-grade, 2/3 the tensor work */
 
 #define CCAB_MAX_VIEWS 8
 
