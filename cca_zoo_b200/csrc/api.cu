@@ -12,6 +12,7 @@
 #include "cholinv.cuh"
 #include "common.cuh"
 #include "dense.cuh"
+#include "ey.cuh"
 #include "fit.cuh"
 #include "moments.cuh"
 #include "syevj.cuh"
@@ -614,6 +615,50 @@ int ccab_als_fit(int kind, int n_views, const int64_t* dims, const double* G, do
   if (rc) return rc;
   return als_fit(kind, L, G, g_scale, n_samples, params, mu, init, k, max_iter, tol, W_out, iters_out, workspace,
                  workspace_bytes, static_cast<cudaStream_t>(stream));
+  CCAB_CATCH
+}
+
+size_t ccab_ey_fit_workspace_bytes(int n_views, const int64_t* dims, int k, int batch) {
+  ColumnLayout L;
+  if (!dims || n_views < 2 || k < 1 || k > kEyMaxK || batch < 0 || batch == 1 || make_layout(n_views, dims, &L))
+    return 0;
+  return ey_fit_workspace_bytes(L, k, batch);
+}
+
+int ccab_ey_fit(int n_views, const int64_t* dims, int k, double c, double learning_rate, double momentum, double tol,
+                int n_steps, const double* cov, int dtype, const void* const* views, const int64_t* ld, int batch,
+                const int32_t* idx, double* state, void* workspace, size_t workspace_bytes, void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(n_views >= 2, "the EY estimators need at least 2 views, got %d", n_views);
+  CCAB_CHECK_ARG(dims && state && workspace, "null pointer argument");
+  CCAB_CHECK_ARG(k >= 1 && k <= kEyMaxK, "k = %d: the EY fit supports 1 <= k <= %d", k, kEyMaxK);
+  CCAB_CHECK_ARG(n_steps >= 0, "bad n_steps %d", n_steps);
+  CCAB_CHECK_ARG(c >= 0.0 && c <= 1.0, "c = %g is outside [0, 1]", c);
+  if (cov) {
+    CCAB_CHECK_ARG(batch == 0, "the covariance route takes batch = 0, got %d", batch);
+  } else {
+    CCAB_CHECK_ARG(batch >= 2, "the mini-batch route needs batch >= 2, got %d", batch);
+    CCAB_CHECK_ARG(views && ld && idx, "null pointer argument");
+    CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
+  }
+  ColumnLayout L;
+  int rc = make_layout(n_views, dims, &L);
+  if (rc) return rc;
+  for (int v = 0; !cov && v < n_views; ++v) {
+    CCAB_CHECK_ARG(views[v], "views[%d] is NULL", v);
+    CCAB_CHECK_ARG(ld[v] >= dims[v], "ld[%d] = %lld < dims[%d] = %lld", v, (long long)ld[v], v, (long long)dims[v]);
+  }
+  rc = require_device();
+  if (rc) return rc;
+  EyParams p;
+  p.k = k;
+  p.n_steps = n_steps;
+  p.batch = cov ? 0 : batch;
+  p.c = c;
+  p.lr = learning_rate;
+  p.momentum = momentum;
+  p.tol = tol;
+  return ey_fit(L, p, cov, dtype, views, ld, idx, state, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
   CCAB_CATCH
 }
 

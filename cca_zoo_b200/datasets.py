@@ -83,4 +83,7 @@ def conftest_views(name):
         return [x1, x2]
     if name == "two_views_test":
         return [rng.standard_normal((20, 10)), rng.standard_normal((20, 8))]
+    if name == "three_correlated_views":       # cca_zoo tests/linear/test_gradient.py:19-26
+        z = rng.standard_normal((300, 2))
+        return [z @ rng.standard_normal((2, p)) + 0.1 * rng.standard_normal((300, p)) for p in (10, 8, 6)]
     raise KeyError(name)

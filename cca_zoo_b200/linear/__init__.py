@@ -5,6 +5,7 @@ from ._gcca import GCCA
 from ._partialcca import PartialCCA
 from ._grcca import GRCCA
 from ._iterative import PLS_ALS, SCCA_ADMM, SCCA_PMD, ParkhomenkoCCA, SCCA_Span
+from .gradient import CCA_EY, MCCA_EY, PLS_EY
 
 __all__ = ["CCA", "rCCA", "PLS", "MCCA", "GCCA", "PartialCCA", "GRCCA", "PLS_ALS", "SCCA_PMD", "ParkhomenkoCCA",
-           "SCCA_Span", "SCCA_ADMM"]
+           "SCCA_Span", "SCCA_ADMM", "PLS_EY", "CCA_EY", "MCCA_EY"]

@@ -609,6 +609,86 @@ def als_fit(cov, dims, n_total, kind: str, params, init, max_iter: int, tol: flo
     return host[:D * k].reshape(D, k).copy(), host[D * k:].view(np.int32)[:k].astype(int).tolist()
 
 
+EY_HEADER = 8      # doubles in front of W and the velocity in the state block of ccab_ey_fit
+EY_MAX_K = 32
+
+
+class EyFit:
+    """One Eckart-Young gradient fit on the device (ccab_ey_fit): the state block (header | W (k x D) | velocity) and
+    the workspace of a route, kept across the chunked calls of one fit.
+
+    ``cov`` (float64 D x D CUDA tensor) selects the covariance route; otherwise ``views`` (CUDA tensors of one dtype,
+    unit column stride) and ``batch`` the mini-batch route.  ``init`` is the D x k float64 host array of initial
+    weights.  ``run(n_steps, idx=None)`` enqueues one call; ``stopped()`` reads the stop flag back (one small copy);
+    ``result()`` copies the state block to the host once and returns (W (D x k float64 numpy), steps taken)."""
+
+    def __init__(self, dims, init, c, learning_rate, momentum, tol, cov=None, views=None, batch=0):
+        import numpy as np
+
+        self.lib = _lib.load()
+        self.dims = [int(d) for d in dims]
+        self.D, self.k = int(sum(self.dims)), int(init.shape[1])
+        self.hyper = (float(c), float(learning_rate), float(momentum), float(tol))
+        self.cov, self.batch = cov, int(batch) if cov is None else 0
+        ref = cov if cov is not None else views[0]
+        _require_cuda(ref, "cov" if cov is not None else "view")
+        self.device = ref.device
+        self._d = _lib.i64_array(self.dims)
+        if cov is not None:
+            if cov.dtype != torch.float64 or tuple(cov.shape) != (self.D, self.D):
+                raise ValueError("the covariance route takes the float64 D x D covariance")
+            self.cov = cov.contiguous()
+            self._views, self._ld, self.dtype = None, None, _lib.F64
+        else:
+            for v in views:
+                _require_cuda(v, "view")
+                if v.dtype != views[0].dtype or v.dtype not in _DT or v.stride(1) != 1 or v.device != self.device:
+                    raise ValueError("the mini-batch route takes CUDA views of one dtype with unit column stride")
+            self.views = views
+            self._views = (C.c_void_p * len(views))(*[v.data_ptr() for v in views])
+            self._ld = _lib.i64_array([v.stride(0) for v in views])
+            self.dtype = _DT[views[0].dtype]
+        nbytes = self.lib.ccab_ey_fit_workspace_bytes(len(self.dims), self._d, self.k, self.batch)
+        if nbytes == 0:
+            raise ValueError(f"ccab_ey_fit does not support widths {self.dims} with k = {self.k} (1 <= k <= "
+                             f"{EY_MAX_K}, 2 to {_lib.MAX_VIEWS} views) and batch = {self.batch}")
+        self.ws = _ws(nbytes, self.device)
+        host = np.zeros(EY_HEADER + 2 * self.D * self.k)
+        host[0] = np.inf
+        host[EY_HEADER:EY_HEADER + self.D * self.k] = np.asarray(init, dtype=np.float64).T.reshape(-1)
+        self.state = torch.from_numpy(host).to(self.device)
+        self._flag = torch.empty(1, dtype=torch.float64, pin_memory=True)
+
+    def run(self, n_steps: int, idx=None):
+        c, lr, mom, tol = self.hyper
+        with torch.cuda.device(self.device):
+            rc = self.lib.ccab_ey_fit(len(self.dims), self._d, self.k, c, lr, mom, tol, int(n_steps),
+                                      _ptr(self.cov), self.dtype, self._views, self._ld, self.batch, _ptr(idx),
+                                      _ptr(self.state), _ptr(self.ws), self.ws.numel(),
+                                      C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        _lib.check(rc, "ccab_ey_fit")
+
+    def stopped(self) -> bool:
+        self._flag.copy_(self.state[2:3])
+        return bool(self._flag[0] != 0.0)
+
+    def result(self):
+        host = self.state.cpu().numpy()
+        W = host[EY_HEADER:EY_HEADER + self.D * self.k].reshape(self.k, self.D).T.copy()
+        return W, int(host[1])
+
+
+def ey_fit(dims, init, c, learning_rate, momentum, tol, cov=None, views=None, batch=0) -> EyFit:
+    """The device state of one Eckart-Young gradient fit (see ``EyFit``)."""
+    return EyFit(dims, init, c, learning_rate, momentum, tol, cov=cov, views=views, batch=batch)
+
+
+def column_sums(view):
+    """Column sums of an (n, d) CUDA tensor as one GEMM with a row of ones (float64 result)."""
+    ones = torch.ones((1, view.shape[0]), dtype=view.dtype, device=view.device)
+    return gemm(ones, view)[0].to(torch.float64)
+
+
 _POW = {None: 0, 1: 0, -1: 1, -0.5: 2}
 
 

@@ -276,6 +276,29 @@ int ccab_als_fit(int kind, int n_views, const int64_t* dims, const double* G, do
                  const double* params, double mu, const double* init, int k, int max_iter, double tol, double* W_out,
                  int* iters_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- the Eckart-Young gradient estimators behind the ABI -------------------------------------------------------------
+ * CCA_EY, PLS_EY (c = 1) and MCCA_EY: up to n_steps momentum steps on the EY loss
+ *   L = -2 tr(C_ey - c V) + tr(Vb Vb),  Vb = (1 - c) V + c B,  B = (1/m) sum_i W_i^T W_i
+ * (vel = momentum * vel - learning_rate * g;  W += vel), ALL in one persistent cooperative launch, asynchronous, no
+ * host synchronisation.  The fit state lives in a caller-owned device block of 8 + 2 * k * D doubles:
+ *   state[0] previous objective (+inf before the first step), state[1] steps taken, state[2] stop flag,
+ *   state[3] |change of the objective| of the last step, state[4..7] reserved (zero),
+ *   then W (k x D: W[x * D + r] is row r of the hstacked weights, column x) and the velocity (same layout).
+ * A step whose |prev_obj - obj| < tol sets the stop flag; once it is set, later steps and later calls do nothing (a
+ * NaN objective never sets it).  Call repeatedly to run a fit in chunks.
+ *   cov        covariance route (full batch): the centred D x D block covariance (device, row-major, float64);
+ *              views / ld / idx are ignored and batch must be 0.
+ *   batch > 1  mini-batch route (cov NULL): step s of this call uses rows idx[s * batch .. (s + 1) * batch) (device
+ *              int32) gathered straight from the raw views (device pointers, all `dtype`, row-major with leading
+ *              dimension ld[i] >= dims[i]); the batch is centred inside the step.
+ * Needs 2 <= n_views <= 8 and 1 <= k <= 32.  Fixed-order reductions only: repeated calls give bit-identical results.
+ * Replaces cca_zoo/linear/gradient/_base.py:113-130 with _derivative / _objective of
+ * cca_zoo/linear/gradient/_cca_ey.py:195-225. */
+size_t ccab_ey_fit_workspace_bytes(int n_views, const int64_t* dims, int k, int batch);
+int ccab_ey_fit(int n_views, const int64_t* dims, int k, double c, double learning_rate, double momentum, double tol,
+                int n_steps, const double* cov, int dtype, const void* const* views, const int64_t* ld, int batch,
+                const int32_t* idx, double* state, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- the deep-CCA objective behind the ABI (any widths) ---------------------------------------------------------
  * ccab_ccaloss_fwd: loss[0] = -|| S11^-1/2 S12 S22^-1/2 ||_F^2 with S_ii = cov(z_i) + eps I, from the moment pass over
  * [z1 z2] (precision as in ccab_moments), a batched Cholesky + inverse and 7 GEMMs; `saved`
