@@ -3,8 +3,9 @@
 //   * moments_wgmma_kernel : Hopper wgmma (TF32, fp32 accumulators in registers), 128 x 128 tiles of the upper
 //     block triangle, split over the sample axis.  A producer / consumer pipeline on mbarriers: TMA loads of the raw
 //     sample slices, two transpose warpgroups that write them as K-major swizzled shared tiles, two wgmma
-//     warpgroups.  Optional 3xTF32 (hi / lo copies in shared memory, 3 MMAs per k-step) for fp32-grade accuracy,
-//     with the two cross terms either in TF32 or as bf16 MMAs (2 instead of 3 units of tensor work).
+//     warpgroups.  Optional 3xTF32 (hi / lo copies in shared memory, 3 MMAs per k-step) for fp32-grade accuracy.
+//   * moments_x3b_pair_kernel : the same pipeline for 3xTF32 with the two cross terms as bf16 MMAs (2 instead of 3
+//     units of tensor work), on 256 x 128 pair tiles: one transposed B block feeds two A blocks.
 //     Column sums are exact fp32 sums of the loaded values.
 //   * moments_simt_kernel : exact FMA (fp32) tile kernel, the non-tensor reference path;
 //     moments_dmma_kernel : float64 inputs on the fp64 tensor pipe (mma.sync m8n8k4.f64).
@@ -88,18 +89,6 @@ float moments_profile_last_ms() {
 // The swizzle makes the raw reads conflict-free for both readers: a transpose warp reads one 128-byte box row, and a
 // fragment load takes samples {0,5,2,7} (then {4,1,6,3}) of a k-step on lanes t = lane % 4 = 0..3, so the 32 lanes
 // hit 32 distinct banks.
-//
-// X3B mode (3xTF32 with bf16 cross terms): hi*hi stays a TF32 MMA per k-step of 8 samples, and lo*hi + hi*lo run as
-// bf16 m64n128k16 MMAs per k16 step of 16 samples, at twice the TF32 rate.  hi = trunc_tf32(x); the bf16 copies are
-// rne_bf16(hi) and rne_bf16(x - hi).  A bf16 k16 step takes its k index in the order of the registers an MMA thread
-// already holds for two TF32 k-steps: logical k 2t, 2t+1, 2t+8, 2t+9 of the step are samples t, t+4, 8+t, 12+t.  (Any
-// sample permutation leaves X^T X unchanged as long as A and B share it.)  So the bf16 A fragment is packed from the
-// TF32 fragment's registers, and chunk e (16 bytes) of a row of the bf16 B tile holds the pairs (8e+t, 8e+t+4),
-// t = 0..3.  The bf16 tile is one 128 x 128-byte K-major tile with 128-byte swizzle: hi in bytes 0..63 of a row (k16
-// steps 0, 1), lo in bytes 64..127.  An operand stage is the TF32 hi tile and this tile, 32 KB as in X3.  The two
-// samples of a pair belong to different parity groups, so an X3B transpose thread (h, m) owns the k16 step h.
-// Per slice of an off-diagonal tile that is 8 TF32 + 8 bf16 MMAs (the tensor time of 16 TF32 MMAs, 24 in X3) and about
-// 160 KB of shared-memory traffic: 32 KB TMA, 16 KB transpose reads, 32 KB stores, 16 KB A fragments, 64 KB B reads.
 struct WgParams {
   CUtensorMap map[kMaxViews];   // view v: {width, rows} fp32, row pitch lds[v], box 32 columns x 32 rows, 128B swizzle
   uint8_t blk_view[kMaxBlocks];
@@ -123,12 +112,12 @@ __device__ __forceinline__ uint32_t raw_offset(int k, int m) {
   return (uint32_t)(m >> 5) * kWgBox + k128_offset(k, (m & 31) >> 2) + (uint32_t)(m & 3) * 4;
 }
 
-// Operand arithmetic of the kernel: one TF32 pass, 3xTF32, 3xTF32 with the cross terms as bf16 MMAs
-enum class K1Mode { TF32, X3, X3B };
+// Operand arithmetic of moments_wgmma_kernel: one TF32 pass, 3xTF32
+enum class K1Mode { TF32, X3 };
 
 template <K1Mode M>
 struct WgCfg {
-  static constexpr int kOps = M == K1Mode::TF32 ? 1 : 2;   // B operand tiles: hi (+ lo, or + bf16 hi | lo)
+  static constexpr int kOps = M == K1Mode::TF32 ? 1 : 2;   // B operand tiles: hi (+ lo)
   static constexpr int kOpStage = kOps * kWgTile;
   static constexpr int kRawStage = 2 * kWgTile;    // raw A block, raw B block
   static constexpr int kOpStages = M == K1Mode::TF32 ? 3 : 2;
@@ -138,11 +127,10 @@ struct WgCfg {
   static constexpr int kSumOff = kBarOff + 2 * (kOpStages + kRawStages) * 8;       // odd column sums
   static constexpr int kSmem = kSumOff + kBlk * 4 + 1024;   // + alignment slack
 };
-static_assert(WgCfg<K1Mode::X3>::kSmem <= 227 * 1024 && WgCfg<K1Mode::TF32>::kSmem <= 227 * 1024 &&
-              WgCfg<K1Mode::X3B>::kSmem <= 227 * 1024, "shared memory per block");
+static_assert(WgCfg<K1Mode::X3>::kSmem <= 227 * 1024 && WgCfg<K1Mode::TF32>::kSmem <= 227 * 1024,
+              "shared memory per block");
 static_assert(WgCfg<K1Mode::X3>::kRawStages > WgCfg<K1Mode::X3>::kOpStages &&
-              WgCfg<K1Mode::TF32>::kRawStages > WgCfg<K1Mode::TF32>::kOpStages &&
-              WgCfg<K1Mode::X3B>::kRawStages > WgCfg<K1Mode::X3B>::kOpStages,
+              WgCfg<K1Mode::TF32>::kRawStages > WgCfg<K1Mode::TF32>::kOpStages,
               "the refill of a raw stage must not wait on the MMA warps' current slice");
 
 template <K1Mode M>
@@ -203,43 +191,21 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
     if (threadIdx.x == 0)
       for (int c = 0; c < min(NR, nch); ++c) issue(c);
 
-    float csum = 0.f;   // column m of a diagonal tile over the 4-sample groups of parity h (X3B: k16 step h)
+    float csum = 0.f;   // column m of a diagonal tile over the 4-sample groups of parity h
     auto transpose = [&](const uint8_t* src, uint8_t* hi, uint8_t* lo, bool sums) {
-      if constexpr (M == K1Mode::X3B) {   // lo: the bf16 tile, hi | lo pairs of k-step e in chunks e | 4 + e
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          const int e = 2 * h + q;   // k-step of 8 samples
-          float v[8], x[8];
+      for (int j = 0; j < kWgKC / 8; ++j) {
+        const int kg = 2 * j + h;
+        float v[4];
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {   // a warp reads one 128-byte box row: conflict-free
-            v[i] = *reinterpret_cast<const float*>(src + raw_offset(8 * e + i, m));
-            x[i] = tf32_hi(v[i]);
-          }
-          *reinterpret_cast<float4*>(hi + k128_offset(m, 2 * e)) = make_float4(x[0], x[1], x[2], x[3]);
-          *reinterpret_cast<float4*>(hi + k128_offset(m, 2 * e + 1)) = make_float4(x[4], x[5], x[6], x[7]);
-          *reinterpret_cast<uint4*>(lo + k128_offset(m, e)) =
-              make_uint4(pack_bf16x2(x[0], x[4]), pack_bf16x2(x[1], x[5]), pack_bf16x2(x[2], x[6]),
-                         pack_bf16x2(x[3], x[7]));
-          *reinterpret_cast<uint4*>(lo + k128_offset(m, 4 + e)) =
-              make_uint4(pack_bf16x2(v[0] - x[0], v[4] - x[4]), pack_bf16x2(v[1] - x[1], v[5] - x[5]),
-                         pack_bf16x2(v[2] - x[2], v[6] - x[6]), pack_bf16x2(v[3] - x[3], v[7] - x[7]));
-          if (sums) csum += ((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]));
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < kWgKC / 8; ++j) {
-          const int kg = 2 * j + h;
-          float v[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e)   // a warp reads one 128-byte box row: conflict-free
-            v[e] = *reinterpret_cast<const float*>(src + raw_offset(4 * kg + e, m));
-          const uint32_t off = k128_offset(m, kg);
-          *reinterpret_cast<float4*>(hi + off) = make_float4(tf32_hi(v[0]), tf32_hi(v[1]), tf32_hi(v[2]), tf32_hi(v[3]));
-          if (X3)
-            *reinterpret_cast<float4*>(lo + off) = make_float4(tf32_residual(v[0]), tf32_residual(v[1]),
-                                                               tf32_residual(v[2]), tf32_residual(v[3]));
-          if (sums) csum += (v[0] + v[1]) + (v[2] + v[3]);
-        }
+        for (int e = 0; e < 4; ++e)   // a warp reads one 128-byte box row: conflict-free
+          v[e] = *reinterpret_cast<const float*>(src + raw_offset(4 * kg + e, m));
+        const uint32_t off = k128_offset(m, kg);
+        *reinterpret_cast<float4*>(hi + off) = make_float4(tf32_hi(v[0]), tf32_hi(v[1]), tf32_hi(v[2]), tf32_hi(v[3]));
+        if (X3)
+          *reinterpret_cast<float4*>(lo + off) = make_float4(tf32_residual(v[0]), tf32_residual(v[1]),
+                                                             tf32_residual(v[2]), tf32_residual(v[3]));
+        if (sums) csum += (v[0] + v[1]) + (v[2] + v[3]);
       }
     };
     for (int c = 0; c < nch; ++c) {
@@ -284,14 +250,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
     // One wgmma group per step, so that the fragment registers of a step are free once its group of the previous
     // slice has retired.  A step is one k-step of 8 samples: a ring of four k-step fragments, 32 registers in 3xTF32
     // mode, with three groups in flight while the next fragments are loaded.  (Two whole-slice fragment sets do not fit
-    // next to the accumulators in the 128 registers a 512-thread CTA compiles to.)  In X3B a step is a k16 step: the
-    // TF32 hi fragments of its two k-steps and the bf16 hi and lo fragments of the k16 MMAs, a ring of two steps (32
-    // registers) with one group in flight.
-    constexpr int KQ = M == K1Mode::X3B ? 2 : 1;                   // k-steps per step
-    constexpr int KS = kWgKC / (8 * KQ);                            // steps per slice
-    constexpr int KR = M == K1Mode::X3B ? 16 : Cfg::kOps * 4;       // fragment registers per step
-    // fragment registers of a step: 0..3 TF32 hi, 4..7 TF32 lo; X3B: 0..3 and 4..7 TF32 hi of its two k-steps,
-    // 8..11 bf16 hi, 12..15 bf16 lo
+    // next to the accumulators in the 128 registers a 512-thread CTA compiles to.)
+    constexpr int KS = kWgKC / 8;          // steps per slice
+    constexpr int KR = Cfg::kOps * 4;      // fragment registers per step: 0..3 TF32 hi, 4..7 TF32 lo
     uint32_t fa[KS][KR] = {};
     for (int c = 0; c < nch; ++c) {
       const int sr = c % NR, so = c % NO;
@@ -306,26 +267,15 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
         wgmma_fence_regs<KR>(fa[kk]);
         // the last step of slice c - 1 has retired with it: hand that slice's operand stage back
         if (kk == KS - 1 && c > 0 && lane == 0) mbar_arrive(&op_empty[(c - 1) % NO]);
-#pragma unroll
-        for (int q = 0; q < KQ; ++q) {
-          const uint8_t* s = a_src + (KQ * kk + q) * 1024;
+        {
+          const uint8_t* s = a_src + kk * 1024;
           const float v00 = *reinterpret_cast<const float*>(s + o00), v01 = *reinterpret_cast<const float*>(s + o01);
           const float v10 = *reinterpret_cast<const float*>(s + o10), v11 = *reinterpret_cast<const float*>(s + o11);
           const float a[4] = {swap ? v01 : v00, swap ? v11 : v10, swap ? v00 : v01, swap ? v10 : v11};
-          float x[4];
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
-            x[i] = tf32_hi(a[i]);
-            fa[kk][4 * q + i] = __float_as_uint(x[i]);
+            fa[kk][i] = __float_as_uint(tf32_hi(a[i]));
             if constexpr (X3) fa[kk][4 + i] = __float_as_uint(tf32_residual(a[i]));
-          }
-          if constexpr (M == K1Mode::X3B) {
-            // bf16 register 2q + r: row g + 8r, samples t (low half) and t + 4 of k-step q of the step
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-              fa[kk][8 + 2 * q + r] = pack_bf16x2(x[r], x[r + 2]);
-              fa[kk][12 + 2 * q + r] = pack_bf16x2(a[r] - x[r], a[r + 2] - x[r + 2]);
-            }
           }
         }
         wgmma_fence_regs<KR>(fa[kk]);
@@ -335,20 +285,13 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
         }
         if (kk == 0) mbar_wait(&op_full[so], (c / NO) & 1);
         wgmma_fence();
-        if constexpr (M == K1Mode::X3B) {   // bf16 tile: hi of k16 step kk at 32 kk, lo at 64 + 32 kk
-          wgmma_bf16_ra<128>(acc, &fa[kk][12], wgmma_desc_k128(b0 + kWgTile + 32 * kk));        // lo * hi
-          wgmma_bf16_ra<128>(acc, &fa[kk][8], wgmma_desc_k128(b0 + kWgTile + 64 + 32 * kk));    // hi * lo
-          wgmma_tf32_ra<128>(acc, &fa[kk][0], wgmma_desc_k128(b0 + 64 * kk));
-          wgmma_tf32_ra<128>(acc, &fa[kk][4], wgmma_desc_k128(b0 + 64 * kk + 32));
-        } else {
-          const uint64_t b_hi = wgmma_desc_k128(b0 + 32 * kk);
-          if constexpr (X3) {
-            const uint64_t b_lo = wgmma_desc_k128(b0 + kWgTile + 32 * kk);
-            wgmma_tf32_ra<128>(acc, &fa[kk][4], b_hi);   // small cross terms first
-            wgmma_tf32_ra<128>(acc, &fa[kk][0], b_lo);
-          }
-          wgmma_tf32_ra<128>(acc, &fa[kk][0], b_hi);
+        const uint64_t b_hi = wgmma_desc_k128(b0 + 32 * kk);
+        if constexpr (X3) {
+          const uint64_t b_lo = wgmma_desc_k128(b0 + kWgTile + 32 * kk);
+          wgmma_tf32_ra<128>(acc, &fa[kk][4], b_hi);   // small cross terms first
+          wgmma_tf32_ra<128>(acc, &fa[kk][0], b_lo);
         }
+        wgmma_tf32_ra<128>(acc, &fa[kk][0], b_hi);
         wgmma_commit();
       }
     }
@@ -367,6 +310,250 @@ __global__ void __launch_bounds__(kWgThreads, 1) moments_wgmma_kernel(const __gr
     }
   }
 }
+
+// =============================================================================================
+// tf32x3b pair-tile kernel
+// =============================================================================================
+// 3xTF32 with the cross terms as bf16 MMAs: hi*hi stays a TF32 MMA per k-step of 8 samples, and lo*hi + hi*lo run as
+// bf16 m64n128k16 MMAs per k16 step of 16 samples, at twice the TF32 rate.  hi = trunc_tf32(x); the bf16 copies are
+// rne_bf16(hi) and rne_bf16(x - hi).  A bf16 k16 step takes its k index in the order of the registers an MMA thread
+// already holds for two TF32 k-steps: logical k 2t, 2t+1, 2t+8, 2t+9 of the step are samples t, t+4, 8+t, 12+t.  (Any
+// sample permutation leaves X^T X unchanged as long as A and B share it.)  So the bf16 A fragment is packed from the
+// TF32 fragment's registers, and chunk e (16 bytes) of a row of the bf16 B tile holds the pairs (8e+t, 8e+t+4),
+// t = 0..3.  The bf16 tile is one 128 x 128-byte K-major tile with 128-byte swizzle: hi in bytes 0..63 of a row (k16
+// steps 0, 1), lo in bytes 64..127.  An operand stage is the TF32 hi tile and this tile, 32 KB.
+//
+// One CTA = one pair tile over one split of the sample axis: A blocks 2i and 2i + 1 against a B block j >= 2i, i.e.
+// 256 x 128 of M, so that each transposed B slice feeds two A blocks.  Pair i has the tiles j = 2i .. nblocks - 1:
+//   * j > 2i + 1 loads A0 | A1 | B (48 KB per raw stage);
+//   * j = 2i + 1: B is A1; both A blocks are loaded, the tile holds sub-tiles (2i, 2i+1) and the diagonal (2i+1, 2i+1);
+//   * j = 2i: B is A0; only A0 is loaded and only the diagonal (2i, 2i) is computed: sub-tile (2i+1, 2i) lies below
+//     the block diagonal, and the second MMA warpgroup idles.  A lone last block (odd nblocks) is this case.
+// The tiles with j in {2i, 2i+1} take the exact fp32 column sums of block j, so each block's sums are written once.
+// For nblocks = 16 that is 72 pair tiles instead of 136 unit tiles.  Three roles meet only on mbarriers:
+//   * thread 0 issues the TMA loads of each slice (as moments_wgmma_kernel) into a ring of raw stages;
+//   * one transpose warpgroup, thread m owning column m of B: the K-major TF32 hi tile and the bf16 hi | lo tile;
+//   * two MMA warpgroups, warpgroup g owning the 128 rows of A block 2i + g as two m64n128 accumulators (128
+//     registers).  A fragments come straight from the raw stage as in moments_wgmma_kernel.  A step is one k16 step
+//     of one 64-row group: 2 TF32 + 2 bf16 MMAs in one wgmma group, four steps per slice, a ring of four steps of
+//     fragment registers (64) with three groups in flight.  Every output element sees the MMAs of the unit-tile
+//     kernel in the same order (per k16 step: lo*hi, hi*lo, hi*hi of its two k-steps), over the same 2048-sample
+//     accumulator runs, so the partials are bit for bit those of 128 x 128 tiles.
+// Per slice of a j > 2i + 1 tile (two unit tiles of MMA work, 2048 tensor clocks) the shared-memory traffic is about
+// 48 KB TMA, 16 KB transpose reads, 32 KB stores, 32 KB A fragments and 128 KB B reads: 128 KB per unit tile instead
+// of 160 KB.
+// At config 2 on an H100 the loads bind it, not shared memory: alone they take 80 % of the MMA time (9.8 GB from L2),
+// and they overlap with the MMAs only in part (DESIGN.md §4).
+constexpr int kPrXpose = 128;                  // one transpose warpgroup (its thread 0 issues the TMA loads)
+constexpr int kPrThreads = kPrXpose + 256;     // + two MMA warpgroups
+struct PairCfg {
+  static constexpr int kOpStage = 2 * kWgTile;    // TF32 hi tile | bf16 hi | lo tile
+  static constexpr int kRawStage = 3 * kWgTile;   // raw A0 | A1 | B
+  static constexpr int kOpStages = 2;
+  static constexpr int kRawStages = 3;
+  static constexpr int kFrag = 4;                 // steps of A fragment registers
+  static constexpr int kBarOff = kOpStages * kOpStage + kRawStages * kRawStage;
+  static constexpr int kSmem = kBarOff + 2 * (kOpStages + kRawStages) * 8 + 1024;   // + alignment slack
+  // registers: 128 x 56 + 256 x 224 = 384 x 168, what the CTA is allocated at launch
+  static constexpr int kXposeRegs = 56, kMmaRegs = 224;
+};
+static_assert(PairCfg::kSmem <= 227 * 1024, "shared memory per block");
+static_assert(PairCfg::kRawStages > PairCfg::kOpStages,
+              "the refill of a raw stage must not wait on the MMA warps' current slice");
+static_assert(kPrXpose * PairCfg::kXposeRegs + 256 * PairCfg::kMmaRegs <= kPrThreads * (65536 / kPrThreads / 8 * 8),
+              "the register budgets must fit in what the CTA is allocated at launch");
+static_assert(4 % PairCfg::kFrag == 0, "a slice is four steps");
+
+// pair tiles of the upper block triangle of nblocks blocks: sum over i of nblocks - 2i
+inline int pair_tiles(int nblocks) {
+  int n = 0;
+  for (int i = 0; 2 * i < nblocks; ++i) n += nblocks - 2 * i;
+  return n;
+}
+
+__global__ void __launch_bounds__(kPrThreads, 1) moments_x3b_pair_kernel(const __grid_constant__ WgParams p) {
+  constexpr int NO = PairCfg::kOpStages, NR = PairCfg::kRawStages, NF = PairCfg::kFrag;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* ops = smem;                              // operand stages (1024-byte aligned: swizzle atoms)
+  uint8_t* raw = smem + NO * PairCfg::kOpStage;     // raw stages
+  uint64_t* raw_full = reinterpret_cast<uint64_t*>(smem + PairCfg::kBarOff);
+  uint64_t* raw_empty = raw_full + NR;
+  uint64_t* op_full = raw_empty + NR;
+  uint64_t* op_empty = op_full + NO;
+
+  int t = blockIdx.x, i = 0, rowlen = p.nblocks;   // pair tile decode
+  while (t >= rowlen) { t -= rowlen; ++i; rowlen -= 2; }
+  const int a0 = 2 * i, bj = a0 + t;
+  const int nload = min(t, 2) + 1;   // raw blocks per slice: A0 (j = 2i); A0, A1 (j = 2i + 1); A0, A1, B
+  const int na = min(nload, 2);      // A blocks with work, one MMA warpgroup each
+  const int bslot = nload - 1;       // where B sits in the raw stage
+  const bool diag = t < 2;           // B is an A block: its column sums
+  const int split = blockIdx.y;
+  const int64_t r0 = (int64_t)split * p.rows_per_split;
+  const int64_t r1 = min(r0 + p.rows_per_split, p.n_rows);
+  const int nch = r1 > r0 ? (int)((r1 - r0 + kWgKC - 1) / kWgKC) : 0;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NR; ++s) {
+      mbar_init(&raw_full[s], 1);
+      mbar_init(&raw_empty[s], kPrXpose + 4 * na);   // every transpose thread and one lane of each working MMA warp
+    }
+    for (int s = 0; s < NO; ++s) {
+      mbar_init(&op_full[s], kPrXpose);
+      mbar_init(&op_empty[s], 4 * na);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (threadIdx.x < kPrXpose) {
+    // ---- TMA issue (thread 0) and the transpose warpgroup ----
+    setmaxnreg_dec<PairCfg::kXposeRegs>();
+    const int m = threadIdx.x;   // column of B
+    auto issue = [&](int c) {
+      const int s = c % NR;
+      const int row = (int)(p.row_base + r0 + (int64_t)c * kWgKC);
+      uint8_t* dst = raw + s * PairCfg::kRawStage;
+      mbar_arrive_expect_tx(&raw_full[s], nload * kWgTile);
+      for (int b = 0; b < nload; ++b) {
+        const int blk = b < 2 ? a0 + b : bj;
+        const CUtensorMap* map = &p.map[p.blk_view[blk]];
+#pragma unroll
+        for (int q = 0; q < kBlk / 32; ++q)
+          tma_load_2d(dst + b * kWgTile + q * kWgBox, map, &raw_full[s], p.blk_col0[blk] + 32 * q, row);
+      }
+    };
+    if (threadIdx.x == 0)
+      for (int c = 0; c < min(NR, nch); ++c) issue(c);
+
+    // column m of a diagonal tile over k16 steps 0 and 1 of each slice, added at the end (as two transpose threads
+    // of a unit tile sum them)
+    float csum[2] = {0.f, 0.f};
+    for (int c = 0; c < nch; ++c) {
+      const int sr = c % NR, so = c % NO;
+      mbar_wait(&raw_full[sr], (c / NR) & 1);
+      mbar_wait(&op_empty[so], ((c / NO) & 1) ^ 1);   // the MMAs of slice c - NO have retired
+      const uint8_t* src = raw + sr * PairCfg::kRawStage + bslot * kWgTile;
+      uint8_t* hi = ops + so * PairCfg::kOpStage;
+      uint8_t* lo = hi + kWgTile;   // the bf16 tile: hi | lo pairs of k-step e in chunks e | 4 + e
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {   // k-step of 8 samples
+        float v[8], x[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {   // a warp reads one 128-byte box row: conflict-free
+          v[k] = *reinterpret_cast<const float*>(src + raw_offset(8 * e + k, m));
+          x[k] = tf32_hi(v[k]);
+        }
+        *reinterpret_cast<float4*>(hi + k128_offset(m, 2 * e)) = make_float4(x[0], x[1], x[2], x[3]);
+        *reinterpret_cast<float4*>(hi + k128_offset(m, 2 * e + 1)) = make_float4(x[4], x[5], x[6], x[7]);
+        *reinterpret_cast<uint4*>(lo + k128_offset(m, e)) =
+            make_uint4(pack_bf16x2(x[0], x[4]), pack_bf16x2(x[1], x[5]), pack_bf16x2(x[2], x[6]),
+                       pack_bf16x2(x[3], x[7]));
+        *reinterpret_cast<uint4*>(lo + k128_offset(m, 4 + e)) =
+            make_uint4(pack_bf16x2(v[0] - x[0], v[4] - x[4]), pack_bf16x2(v[1] - x[1], v[5] - x[5]),
+                       pack_bf16x2(v[2] - x[2], v[6] - x[6]), pack_bf16x2(v[3] - x[3], v[7] - x[7]));
+        if (diag) csum[e >> 1] += ((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]));
+      }
+      fence_proxy_async_smem();   // the generic-proxy stores become visible to wgmma (async proxy)
+      mbar_arrive(&raw_empty[sr]);
+      mbar_arrive(&op_full[so]);
+      // Refill the raw stage of slice c - NO + 1: the MMA warps hand it back as they load its last A fragments, about
+      // when they hand back the operand stage of slice c - NO (seen above), so this wait is short.
+      const int rf = c + NR - NO + 1;
+      if (threadIdx.x == 0 && rf >= NR && rf < nch) {
+        mbar_wait(&raw_empty[rf % NR], (rf / NR - 1) & 1);
+        issue(rf);
+      }
+    }
+    if (diag) p.partial_sum[(size_t)split * p.Dp + bj * kBlk + m] = csum[0] + csum[1];
+  } else {
+    // ---- MMA warpgroups ----
+    setmaxnreg_inc<PairCfg::kMmaRegs>();
+    const int g = (threadIdx.x - kPrXpose) >> 7;   // A block a0 + g
+    if (g >= na) return;                          // sub-tile below the block diagonal
+    const int lane = threadIdx.x & 31, t4 = lane & 3, warp = (threadIdx.x >> 5) & 3;
+    // Raw-stage offsets of this thread's A fragment elements in k-step 0 of row group 0, as in moments_wgmma_kernel
+    // (k-step kk adds kk * 1024, row group 1 (rows + 64) two boxes)
+    const int m = warp * 16 + (lane >> 2);
+    const int kx = t4 ^ ((t4 & 1) << 2);
+    const bool swap = t4 & 1;
+    const uint32_t o00 = raw_offset(kx, m), o01 = raw_offset(kx ^ 4, m);
+    const uint32_t o10 = raw_offset(kx, m + 8), o11 = raw_offset(kx ^ 4, m + 8);
+    float acc[2][64];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+#pragma unroll
+      for (int k = 0; k < 64; ++k) acc[r][k] = 0.f;
+      wgmma_fence_regs<64>(acc[r]);   // keeps the zeroing out of the wgmma pipeline
+    }
+    // fragment registers of a step: 0..3 and 4..7 TF32 hi of its two k-steps, 8..11 bf16 hi, 12..15 bf16 lo
+    uint32_t fa[NF][16] = {};
+    for (int c = 0; c < nch; ++c) {
+      const int sr = c % NR, so = c % NO;
+      mbar_wait(&raw_full[sr], (c / NR) & 1);
+      const uint8_t* a_src = raw + sr * PairCfg::kRawStage + g * kWgTile;
+      const uint32_t b0 = smem_u32(ops + so * PairCfg::kOpStage);
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {   // step s: k16 step kk of row group r
+        const int kk = s >> 1, r = s & 1, f = s % NF;
+        wgmma_wait<NF - 1>();   // the group that last read fa[f] has retired
+        wgmma_fence_regs<16>(fa[f]);
+        // ... and with it the last step of slice c - 1: hand that slice's operand stage back
+        if (s == NF - 1 && c > 0 && lane == 0) mbar_arrive(&op_empty[(c - 1) % NO]);
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const uint8_t* src = a_src + (2 * kk + q) * 1024 + r * 2 * kWgBox;
+          const float v00 = *reinterpret_cast<const float*>(src + o00), v01 = *reinterpret_cast<const float*>(src + o01);
+          const float v10 = *reinterpret_cast<const float*>(src + o10), v11 = *reinterpret_cast<const float*>(src + o11);
+          const float a[4] = {swap ? v01 : v00, swap ? v11 : v10, swap ? v00 : v01, swap ? v10 : v11};
+          float x[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            x[k] = tf32_hi(a[k]);
+            fa[f][4 * q + k] = __float_as_uint(x[k]);
+          }
+          // bf16 register 2q + h: row + 8h, samples t (low half) and t + 4 of k-step q of the step
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            fa[f][8 + 2 * q + h] = pack_bf16x2(x[h], x[h + 2]);
+            fa[f][12 + 2 * q + h] = pack_bf16x2(a[h] - x[h], a[h + 2] - x[h + 2]);
+          }
+        }
+        wgmma_fence_regs<16>(fa[f]);
+        if (s == 3) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&raw_empty[sr]);   // every lane of the warp has read the slice's A fragments
+        }
+        if (s == 0) mbar_wait(&op_full[so], (c / NO) & 1);
+        wgmma_fence();
+        // bf16 tile: hi of k16 step kk at 32 kk, lo at 64 + 32 kk
+        wgmma_bf16_ra<128>(acc[r], &fa[f][12], wgmma_desc_k128(b0 + kWgTile + 32 * kk));        // lo * hi
+        wgmma_bf16_ra<128>(acc[r], &fa[f][8], wgmma_desc_k128(b0 + kWgTile + 64 + 32 * kk));    // hi * lo
+        wgmma_tf32_ra<128>(acc[r], &fa[f][0], wgmma_desc_k128(b0 + 64 * kk));
+        wgmma_tf32_ra<128>(acc[r], &fa[f][4], wgmma_desc_k128(b0 + 64 * kk + 32));
+        wgmma_commit();
+      }
+    }
+    wgmma_wait_all();
+    wgmma_fence_regs<64>(acc[0]);
+    wgmma_fence_regs<64>(acc[1]);
+
+    // ---- epilogue: fragments -> partial slab of this split ----
+    float* P = p.partial + (size_t)split * p.Dp * p.Dp;
+    const int col0 = bj * kBlk + 2 * t4;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row0 = (a0 + g) * kBlk + r * 64 + m;
+#pragma unroll
+      for (int k = 0; k < 64; k += 2) {
+        const int row = row0 + 8 * ((k >> 1) & 1), col = col0 + 8 * (k >> 2);
+        *reinterpret_cast<float2*>(P + (size_t)row * p.Dp + col) = make_float2(acc[r][k], acc[r][k + 1]);
+      }
+    }
+  }
+}
+
 // =============================================================================================
 // exact SIMT kernel (fp32 / fp64), 64x64 tiles inside the same padded tile space
 // =============================================================================================
@@ -680,7 +867,8 @@ TcPlan plan_tc(const ColumnLayout& L, int64_t n_rows, int mode) {
   TcPlan P;
   P.total_chunks = (int)ceil_div(n_rows, kWgKC);
   P.ntiles = L.nblocks * (L.nblocks + 1) / 2;
-  // about four waves of CTAs, so that the tile count does not leave a mostly idle last wave
+  // about four waves of CTAs, so that the tile count does not leave a mostly idle last wave.  Counted in 128 x 128
+  // unit tiles also for the pair-tile kernel of mode 3, so that every mode splits the sample axis alike.
   int S = (int)ceil_div(4 * sm_count(), P.ntiles);
   int max_splits = 64;
   if (x3) {
@@ -843,6 +1031,13 @@ int launch_wgmma(dim3 grid, const WgParams& prm, cudaStream_t stream) {
   return 0;
 }
 
+int launch_x3b_pair(int num_splits, const WgParams& prm, cudaStream_t stream) {
+  CCAB_CUDA(cudaFuncSetAttribute(moments_x3b_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 PairCfg::kSmem));
+  moments_x3b_pair_kernel<<<dim3(pair_tiles(prm.nblocks), num_splits), kPrThreads, PairCfg::kSmem, stream>>>(prm);
+  return 0;
+}
+
 // One pass over rows [row_base, row_base + n_rows).  Its splits end on multiples of 32 rows from row_base, and a pass
 // that is not the last ends on a multiple of 2048, so no slice reads rows of the next pass.
 int moments_tf32_pass(const ColumnLayout& L, WgParams& prm, int64_t row_base, int64_t n_rows, int mode,
@@ -863,7 +1058,7 @@ int moments_tf32_pass(const ColumnLayout& L, WgParams& prm, int64_t row_base, in
   prm.Dp = L.Dp;
   dim3 grid(P.ntiles, P.num_splits);
   if (g_prof_on) cudaEventRecord(g_prof_e0, stream);
-  int rc = mode == 3   ? launch_wgmma<K1Mode::X3B>(grid, prm, stream)
+  int rc = mode == 3   ? launch_x3b_pair(P.num_splits, prm, stream)
            : mode != 0 ? launch_wgmma<K1Mode::X3>(grid, prm, stream)
                        : launch_wgmma<K1Mode::TF32>(grid, prm, stream);
   if (rc) return rc;
