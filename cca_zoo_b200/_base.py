@@ -76,6 +76,8 @@ class BaseModel(BaseEstimator, ABC):
     _covariance_always_centred: ClassVar[bool] = False
     #: GCCA with ``center=False`` needs both: np.cov for the regularised blocks, raw products for the rest
     _wants_second_moment: ClassVar[bool] = False
+    #: SCCA_IPLS with ``center=False`` carries the column means of the views through its deflation
+    _wants_column_means: ClassVar[bool] = False
 
     def __init__(self, latent_dimensions: int = 1, center: bool = True, precision: str = "tf32x3b",
                  device=None) -> None:
@@ -226,6 +228,8 @@ class BaseModel(BaseEstimator, ABC):
         self.n_samples_ = n_total
         off = np.concatenate([[0], np.cumsum(dims)]).astype(int)
         mean_np = mean.to(torch.float64).cpu().numpy()
+        if self._wants_column_means:
+            self._column_means = mean_np if centred else ops.column_means(mom, dims, n_total)
         np_dtype = np.float32 if in_dtype == torch.float32 else np.float64
         if self.center:
             self.means_ = [mean_np[off[i]:off[i + 1]].astype(np_dtype) for i in range(len(dims))]

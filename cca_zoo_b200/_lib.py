@@ -71,6 +71,7 @@ SIGNATURES = {
     "ccab_mcca_fit": (C.c_int, [C.c_int, C.c_int, _i64p, _vp, _vp, C.c_double, C.c_int, C.POINTER(C.c_double),
                                 C.c_double, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp, C.c_size_t, _vp]),
     "ccab_als_fit_workspace_bytes": (C.c_size_t, [C.c_int, _i64p]),
+    "ccab_als_regression_workspace_bytes": (C.c_size_t, [C.c_int, _i64p]),
     "ccab_als_fit": (C.c_int, [C.c_int, C.c_int, _i64p, _vp, C.c_double, C.c_double, C.POINTER(C.c_double), C.c_double,
                                _vp, C.c_int, C.c_int, C.c_double, _vp, _vp, _vp, C.c_size_t, _vp]),
     "ccab_ey_fit_workspace_bytes": (C.c_size_t, [C.c_int, _i64p, C.c_int, C.c_int]),

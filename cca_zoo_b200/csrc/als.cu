@@ -12,15 +12,30 @@
 // steps, the convergence test) runs on CTA 0, and grid barriers separate the phases.  Every reduction has a fixed
 // order (warp butterflies, block trees, sums over rows in row order), so repeated fits are bit-identical.
 //
+// ElasticCCA / SCCA_IPLS (kinds 5, 6) replace the thresholding by a penalised regression of view i on the target,
+//   min_w  1/2 w^T Q_i w - b_i^T w + lam_i ||w||_1,   Q_i = G_ii / n + rho_i I,   b_i = X_i^T t / (||t|| n),
+// lam_i = alpha_i l1_i, rho_i = alpha_i (1 - l1_i) (sklearn's Lasso / ElasticNet objectives over n) or alpha_i / n
+// (Ridge, l1_i = 0: ||y - X w||^2 + alpha ||w||^2).  The target
+// of ElasticCCA includes view i itself.  CTA 0 solves it:
+//   lam_i == 0   w = V (Lam / n + rho)^+ V^T b with the eigendecomposition G_ii = V Lam V^T of this dimension
+//                (jacobi_solve on the host side, once per dimension): the minimum-norm solution when Q_i is singular
+//                (always from the second dimension on at alpha = 0: deflation maps the previous w_i to zero);
+//   lam_i > 0    cyclic coordinate descent from the current w_i on the rows of G_ii, the gradient Q w - b recomputed
+//                exactly after every sweep, until the KKT residual is <= kKktTol * max(1, ||b||_inf).
+// SCCA_IPLS then divides by the population std of X_i w, sqrt(w^T G_ii w / n - (mu_i^T w)^2), mu_i the column means
+// of the (deflated) view, deflated with the view (mu_i <- mu_i - (mu_i^T w_i) a_i / s_i).
+//
 // Traffic of one Gauss-Seidel sweep: the update of view i reads the rows of block i (p_i x D), the diagonal block
 // product with the new w_i (p_i x p_i) is read in the phase of view i+1 -- G once per sweep.  An ADMM iteration
 // (Jacobi order) reads G once.
 #include <cooperative_groups.h>
 
 #include <algorithm>
+#include <cstring>
 
 #include "als.cuh"
 #include "common.cuh"
+#include "syevj.cuh"
 
 namespace ccab {
 namespace cg = cooperative_groups;
@@ -29,13 +44,20 @@ namespace {
 
 constexpr int kThreads = 1024;
 constexpr int kWarps = kThreads / 32;
+constexpr int kRegThreads = 512;  // CTA size of the regression kinds
 constexpr int kBisect = 50;  // halvings of the PMD threshold interval (cca_zoo/linear/_iterative.py:246)
+constexpr double kKktTol = 1e-12;  // regression kinds: KKT residual bound relative to max(1, ||b||_inf)
+// coordinate-descent sweeps per sub-problem at most: the max_iter of the reference's sklearn Lasso / ElasticNet.  A
+// sub-problem that does not reach kKktTol in them is reported (negated sweep count of its dimension).
+constexpr int kCdSweeps = 1000;
 
 struct AlsArgs {
   int kind, m, D, k, d, max_iter;
   int off[kMaxViews + 1];
   double param[kMaxViews];  // PMD: L1 bound tau*sqrt(p); Parkhomenko / ADMM: tau; Span: span
-  double mu, tol, n;
+  double rho[kMaxViews], lam[kMaxViews];  // ElasticCCA / IPLS: alpha (1 - l1), alpha l1
+  double mu, tol, n;  // mu: ADMM penalty; regression kinds: the relative eigenvalue cut of the lam == 0 solve
+  int maxp;                                // widest view (the dynamic shared memory holds 3 vectors of it)
   const double* G;     // workspace copy (deflated between dimensions)
   const double* init;  // k x D initial weights (unit per view)
   double* W_out;       // D x k
@@ -49,7 +71,13 @@ struct AlsArgs {
   double* P;           // m x m
   double* fro;         // m   ||G_ii||_F
   int* done;           // convergence flag of the current sweep
+  const double* V;     // regression kinds, lam == 0: eigenvectors of G_ii as rows, p_i x p_i at V + voff[i]
+  const double* ev;    // D: eigenvalues of G_ii (descending per view)
+  double* colmean;     // D: IPLS column means of the deflated views
+  size_t voff[kMaxViews];
 };
+
+
 
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
@@ -63,6 +91,8 @@ __device__ __forceinline__ double warp_max(double v) {
 }
 
 // Block-wide sum (or max), returned to every thread; fixed order: per-thread partial, warp butterfly, warp 0 tree.
+// A CTA of fewer than kWarps warps must zero red[] once first: the slots of its missing warps then stay 0 (the regression
+// kinds only take maxima of non-negative values).
 template <bool MAX>
 __device__ double block_reduce(double v, double* red) {
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -137,19 +167,126 @@ __device__ void all_pairs(const AlsArgs& a, double* red) {
 
 // CTA 0: xs[0..p) = X_i^T t / ||t|| (unnormalised when ||t|| <= 1e-12, as the reference)
 __device__ void target(const AlsArgs& a, int i, double* xs) {
+  const bool self = a.kind == kAlsElastic;  // ElasticCCA: the sum of ALL views' scores
   double tn2 = 0.0;
   for (int j = 0; j < a.m; ++j)
     for (int l = 0; l < a.m; ++l)
-      if (j != i && l != i) tn2 += a.P[j * a.m + l];
+      if (self || (j != i && l != i)) tn2 += a.P[j * a.m + l];
   const double tn = sqrt(fmax(tn2, 0.0));
   const int o = a.off[i], p = a.off[i + 1] - o;
   for (int r = threadIdx.x; r < p; r += blockDim.x) {
     double x = 0.0;
     for (int j = 0; j < a.m; ++j)
-      if (j != i) x += a.R[(size_t)j * a.D + o + r];
+      if (self || j != i) x += a.R[(size_t)j * a.D + o + r];
     xs[r] = tn > 1e-12 ? x / tn : x;
   }
   __syncthreads();
+}
+
+// CTA 0: y[r] = sum_c Gd[r * ld + c] x[c] for r < p (one warp per row, lanes over columns)
+__device__ void cta_matvec(const double* Gd, int ld, int p, const double* x, double* y) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  for (int r = wid; r < p; r += (int)(blockDim.x >> 5)) {
+    const double* g = Gd + (size_t)r * ld;
+    double s0 = 0.0, s1 = 0.0;
+    int c = lane;
+    for (; c + 32 < p; c += 64) {
+      s0 = fma(__ldg(g + c), x[c], s0);
+      s1 = fma(__ldg(g + c + 32), x[c + 32], s1);
+    }
+    if (c < p) s0 = fma(__ldg(g + c), x[c], s0);
+    const double s = warp_sum(s0 + s1);
+    if (lane == 0) y[r] = s;
+  }
+  __syncthreads();
+}
+
+// CTA 0: the largest KKT residual of min 1/2 w^T Q w - b^T w + lam ||w||_1 at w, g = Q w - b
+__device__ double kkt_residual(const double* w, const double* g, int p, double lam, double* red) {
+  double r = 0.0;
+  for (int c = threadIdx.x; c < p; c += blockDim.x)
+    r = fmax(r, w[c] != 0.0 ? fabs(g[c] + copysign(lam, w[c])) : fmax(fabs(g[c]) - lam, 0.0));
+  return block_reduce<true>(r, red);
+}
+
+// CTA 0: the penalised regression of one view (see the header) on its diagonal block Gd (p x p, leading dimension ld),
+// V / ev its eigenvectors (rows) / eigenvalues, w0 its current weights, cm its column means.  In: xs = X_i^T t / ||t||;
+// out: xs = the new w_i.  u, g: scratch vectors of p doubles in shared memory.
+__device__ void regress(int kind, const double* Gd, int ld, int p, double n, double rho, double lam, double rcond,
+                        const double* V, const double* ev, const double* w0, const double* cm, double* xs,
+                        double* u, double* g, double* red, double* bcast, int* fail) {
+  double bmax = 0.0;
+  for (int r = threadIdx.x; r < p; r += blockDim.x) {
+    xs[r] /= n;  // b
+    bmax = fmax(bmax, fabs(xs[r]));
+  }
+  bmax = block_reduce<true>(bmax, red);
+  if (lam == 0.0) {
+    // w = V diag(1 / mu_k) V^T b over the eigenvalues mu_k = ev_k / n + rho above rcond * mu_max
+    const double cut = rcond * fmax(ev[0] / n + rho, 0.0);
+    cta_matvec(V, p, p, xs, u);
+    for (int k = threadIdx.x; k < p; k += blockDim.x) {
+      const double mk = ev[k] / n + rho;
+      u[k] = mk > cut ? u[k] / mk : 0.0;
+    }
+    __syncthreads();
+    for (int r = threadIdx.x; r < p; r += blockDim.x) {
+      double s = 0.0;
+      for (int k = 0; k < p; ++k) s = fma(V[(size_t)k * p + r], u[k], s);
+      g[r] = s;
+    }
+    __syncthreads();
+    for (int r = threadIdx.x; r < p; r += blockDim.x) xs[r] = g[r];
+    __syncthreads();
+  } else {
+    // cyclic coordinate descent on Q_i from the current w_i (u holds w, g the gradient Q w - b)
+    const double tol = kKktTol * fmax(1.0, bmax);
+    for (int r = threadIdx.x; r < p; r += blockDim.x) u[r] = w0[r];
+    __syncthreads();
+    for (int sweep = 0;; ++sweep) {
+      cta_matvec(Gd, ld, p, u, g);
+      for (int r = threadIdx.x; r < p; r += blockDim.x) g[r] = g[r] / n + rho * u[r] - xs[r];
+      __syncthreads();
+      if (kkt_residual(u, g, p, lam, red) <= tol) break;
+      if (sweep == kCdSweeps) {
+        if (threadIdx.x == 0) *fail = 1;
+        break;
+      }
+      for (int j = 0; j < p; ++j) {
+        if (threadIdx.x == 0) {
+          const double q = Gd[(size_t)j * ld + j] / n + rho;
+          const double wj = u[j];
+          const double nw = q > 0.0 ? soft(wj * q - g[j], lam) / q : 0.0;
+          bcast[0] = nw - wj;
+          u[j] = nw;
+        }
+        __syncthreads();
+        const double dl = bcast[0];
+        if (dl != 0.0) {
+          const double* row = Gd + (size_t)j * ld;
+          for (int r = threadIdx.x; r < p; r += blockDim.x) g[r] = fma(dl, row[r] / n + (r == j ? rho : 0.0), g[r]);
+        }
+        __syncthreads();
+      }
+    }
+    for (int r = threadIdx.x; r < p; r += blockDim.x) xs[r] = u[r];
+    __syncthreads();
+  }
+  if (kind == kAlsIpls) {
+    // divide by the population std of the score X_i w when it exceeds 1e-12
+    cta_matvec(Gd, ld, p, xs, u);
+    double q = 0.0, mw = 0.0;
+    for (int r = threadIdx.x; r < p; r += blockDim.x) {
+      q = fma(xs[r], u[r], q);
+      mw = fma(cm[r], xs[r], mw);
+    }
+    q = block_reduce<false>(q, red);
+    mw = block_reduce<false>(mw, red);
+    const double sd = sqrt(fmax(q / n - mw * mw, 0.0));
+    if (sd > 1e-12)
+      for (int r = threadIdx.x; r < p; r += blockDim.x) xs[r] /= sd;
+    __syncthreads();
+  }
 }
 
 // CTA 0: xs /= ||xs|| when the norm exceeds 1e-12
@@ -195,10 +332,13 @@ struct Smem {
   unsigned hist[256];
   unsigned long long sel[2];
   double dmax;
+  double bcast;
+  int cd_fail;  // a coordinate descent of this dimension stopped at kCdSweeps
 };
 
 // CTA 0: Gauss-Seidel update of view i from R[j][rows of i] (j != i); `pend` >= 0 names the view whose diagonal
 // product R[pend][rows of pend] was formed with its new weights in the phase just finished.
+template <bool REG>
 __device__ void gs_update(const AlsArgs& a, int i, int pend, double* xs, Smem& sm) {
   if (pend >= 0) {
     double s = 0.0;
@@ -221,6 +361,9 @@ __device__ void gs_update(const AlsArgs& a, int i, int pend, double* xs, Smem& s
         if (!(fabs(xs[r]) >= thr)) xs[r] = 0.0;
       __syncthreads();
     }
+  } else if (REG) {
+    regress(a.kind, a.G + (size_t)o * a.D + o, a.D, p, a.n, a.rho[i], a.lam[i], a.mu, a.V + a.voff[i], a.ev + o,
+            a.w + o, a.colmean + o, xs, xs + a.maxp, xs + 2 * a.maxp, sm.red, &sm.bcast, &sm.cd_fail);
   } else if (a.kind == kAlsPmd) {
     double l1 = 0.0, mx = 0.0;
     for (int r = threadIdx.x; r < p; r += blockDim.x) {
@@ -243,7 +386,7 @@ __device__ void gs_update(const AlsArgs& a, int i, int pend, double* xs, Smem& s
       __syncthreads();
     }
   }
-  normalise(xs, p, sm.red);
+  if (!REG) normalise(xs, p, sm.red);
   double dd = 0.0;
   for (int r = threadIdx.x; r < p; r += blockDim.x) {
     const double e = xs[r] - a.w[o + r];
@@ -296,13 +439,19 @@ __device__ void admm_update(const AlsArgs& a, double* xs, Smem& sm) {
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(kThreads, 1) als_dimension(AlsArgs a) {
+// REG: the regression kinds (ElasticCCA, SCCA_IPLS); a separate instantiation keeps their solver out of the register
+// allocation of the other kinds, and its 512-thread CTAs give the solver 128 registers
+template <bool REG>
+__global__ void __launch_bounds__(REG ? kRegThreads : kThreads, 1) als_dimension(AlsArgs a) {
   extern __shared__ double xs[];  // CTA 0: the vector of the view being updated
   __shared__ Smem sm;
   cg::grid_group grid = cg::this_grid();
   const bool lead = blockIdx.x == 0;
   const unsigned all = (1u << a.m) - 1u;
   const bool admm = a.kind == kAlsAdmm;
+  if (REG)
+    for (int t = threadIdx.x; t <= kWarps; t += blockDim.x) sm.red[t] = 0.0;  // see block_reduce
+  if (REG && threadIdx.x == 0) sm.cd_fail = 0;
 
   for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < a.D; r += gridDim.x * blockDim.x) {
     const double v = a.init[(size_t)a.d * a.D + r];
@@ -339,11 +488,12 @@ __global__ void __launch_bounds__(kThreads, 1) als_dimension(AlsArgs a) {
         const bool fresh = it == 0 && i == 0;  // R of view 0 comes from the full pass
         if (!fresh) {
           // rows of view i against the other blocks, and the diagonal block of the view just updated
-          matvec(a, a.off[i], a.off[i + 1] - a.off[i], all & ~(1u << i), a.off[prev], a.off[prev + 1] - a.off[prev],
-                 1u << prev, false);
+          // (ElasticCCA: view i's own block too, its target includes X_i w_i)
+          matvec(a, a.off[i], a.off[i + 1] - a.off[i], REG && a.kind == kAlsElastic ? all : all & ~(1u << i), a.off[prev],
+                 a.off[prev + 1] - a.off[prev], 1u << prev, false);
           grid.sync();
         }
-        if (lead) gs_update(a, i, fresh ? -1 : prev, xs, sm);
+        if (lead) gs_update<REG>(a, i, fresh ? -1 : prev, xs, sm);
         if (i + 1 < a.m) grid.sync();
       }
     }
@@ -365,7 +515,15 @@ __global__ void __launch_bounds__(kThreads, 1) als_dimension(AlsArgs a) {
         a.W_out[(size_t)r * a.k + a.d] = a.w[r];
       }
     }
-    if (threadIdx.x == 0) a.iters_out[a.d] = iters;
+    if (REG && a.kind == kAlsIpls)  // deflate the column means with the view: mu_i <- mu_i - (mu_i^T w_i) f_i
+      for (int i = 0; i < a.m; ++i) {
+        double s = 0.0;
+        for (int r = a.off[i] + threadIdx.x; r < a.off[i + 1]; r += blockDim.x) s = fma(a.colmean[r], a.w[r], s);
+        s = block_reduce<false>(s, sm.red);
+        for (int r = a.off[i] + threadIdx.x; r < a.off[i + 1]; r += blockDim.x) a.colmean[r] -= s * a.f[r];
+        __syncthreads();
+      }
+    if (threadIdx.x == 0) a.iters_out[a.d] = REG && sm.cd_fail ? -iters : iters;
   }
 }
 
@@ -399,10 +557,10 @@ __global__ void als_scale_copy(const double* __restrict__ src, double* __restric
 }
 
 struct AlsWorkspace {
-  size_t g, r, w, z, eta, f, rowsq, p, fro, done, total;  // byte offsets
+  size_t g, r, w, z, eta, f, rowsq, p, fro, done, v, ev, colmean, jac, total;  // byte offsets
 };
 
-AlsWorkspace als_workspace(const ColumnLayout& L) {
+AlsWorkspace als_workspace(const ColumnLayout& L, bool reg) {
   auto al = [](size_t x) { return (x + 255) / 256 * 256; };
   const size_t D = (size_t)L.D, m = (size_t)L.n_views;
   AlsWorkspace w;
@@ -416,35 +574,51 @@ AlsWorkspace als_workspace(const ColumnLayout& L) {
   w.p = w.rowsq + al(8 * D);
   w.fro = w.p + al(8 * kMaxViews * kMaxViews);
   w.done = w.fro + al(8 * kMaxViews);
-  w.total = w.done + 256;
+  w.v = w.ev = w.colmean = w.jac = w.total = w.done + 256;
+  if (!reg) return w;
+  // regression kinds only: the eigenvectors of every G_ii, the eigenvalues, the IPLS column means, the eigensolver's
+  size_t vv = 0, jac = 0;
+  for (int i = 0; i < L.n_views; ++i) {
+    vv += (size_t)L.dims[i] * L.dims[i];
+    jac = std::max(jac, jacobi_workspace_bytes<double>(L.dims[i], L.dims[i], 1));
+  }
+  w.ev = w.v + al(8 * vv);
+  w.colmean = w.ev + al(8 * D);
+  w.jac = w.colmean + al(8 * D);
+  w.total = w.jac + al(jac);
   return w;
 }
 
 }  // namespace
 
-size_t als_fit_workspace_bytes(const ColumnLayout& L) { return als_workspace(L).total + 256; }
+size_t als_fit_workspace_bytes(const ColumnLayout& L, bool regression) {
+  return als_workspace(L, regression).total + 256;
+}
 
 int als_fit(int kind, const ColumnLayout& L, const double* G, double g_scale, double n_samples, const double* params,
             double mu, const double* init, int k, int max_iter, double tol, double* W_out, int* iters_out, void* ws,
             size_t ws_bytes, cudaStream_t stream) {
-  CCAB_CHECK_ARG(ws_bytes >= als_fit_workspace_bytes(L), "workspace too small: %zu < %zu", ws_bytes,
-                 als_fit_workspace_bytes(L));
+  const bool reg = kind == kAlsElastic || kind == kAlsIpls;
+  CCAB_CHECK_ARG(ws_bytes >= als_fit_workspace_bytes(L, reg), "workspace too small: %zu < %zu", ws_bytes,
+                 als_fit_workspace_bytes(L, reg));
   int maxp = 0;
   for (int v = 0; v < L.n_views; ++v) maxp = L.dims[v] > maxp ? L.dims[v] : maxp;
-  const size_t smem = (size_t)maxp * sizeof(double);
+  const size_t smem = (size_t)maxp * sizeof(double) * (reg ? 3 : 1);
   int dev = 0, sms = 0, optin = 0;
   CCAB_CUDA(cudaGetDevice(&dev));
   CCAB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   CCAB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   CCAB_CHECK_ARG(smem + sizeof(Smem) <= (size_t)optin, "a view of %d features does not fit the shared memory of the ALS kernel",
                  maxp);
-  CCAB_CUDA(cudaFuncSetAttribute(als_dimension, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const void* kern = reg ? (const void*)als_dimension<true> : (const void*)als_dimension<false>;
+  CCAB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int per_sm = 0;
-  CCAB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, als_dimension, kThreads, smem));
+  const int threads = reg ? kRegThreads : kThreads;
+  CCAB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
   CCAB_CHECK_ARG(per_sm >= 1, "the ALS kernel cannot be resident on this device");
 
   uintptr_t base = ((uintptr_t)ws + 255) / 256 * 256;
-  const AlsWorkspace o = als_workspace(L);
+  const AlsWorkspace o = als_workspace(L, reg);
   AlsArgs a;
   a.kind = kind;
   a.m = L.n_views;
@@ -452,9 +626,17 @@ int als_fit(int kind, const ColumnLayout& L, const double* G, double g_scale, do
   a.k = k;
   a.max_iter = max_iter;
   for (int v = 0; v <= L.n_views; ++v) a.off[v] = L.coff[v];
-  for (int v = 0; v < kMaxViews; ++v) a.param[v] = 0.0;
-  for (int v = 0; v < L.n_views; ++v)
-    a.param[v] = kind == kAlsPmd ? params[v] * sqrt((double)L.dims[v]) : (kind == kAlsPls ? 0.0 : params[v]);
+  a.maxp = maxp;
+  for (int v = 0; v < kMaxViews; ++v) a.param[v] = a.rho[v] = a.lam[v] = 0.0;
+  for (int v = 0; v < L.n_views; ++v) {
+    if (reg) {
+      // Ridge (l1 = 0) minimises ||y - X w||^2 + alpha ||w||^2, not divided by n
+      a.rho[v] = params[2 * v + 1] == 0.0 ? params[2 * v] / n_samples : params[2 * v] * (1.0 - params[2 * v + 1]);
+      a.lam[v] = params[2 * v] * params[2 * v + 1];
+    } else {
+      a.param[v] = kind == kAlsPmd ? params[v] * sqrt((double)L.dims[v]) : (kind == kAlsPls ? 0.0 : params[v]);
+    }
+  }
   a.mu = mu;
   a.tol = tol;
   a.n = n_samples;
@@ -472,6 +654,19 @@ int als_fit(int kind, const ColumnLayout& L, const double* G, double g_scale, do
   a.P = reinterpret_cast<double*>(base + o.p);
   a.fro = reinterpret_cast<double*>(base + o.fro);
   a.done = reinterpret_cast<int*>(base + o.done);
+  double* V = reinterpret_cast<double*>(base + o.v);
+  double* ev = reinterpret_cast<double*>(base + o.ev);
+  a.V = V;
+  a.ev = ev;
+  a.colmean = reinterpret_cast<double*>(base + o.colmean);
+  bool need_eig = false;
+  for (int v = 0, acc = 0; v < L.n_views; ++v) {
+    a.voff[v] = (size_t)acc;
+    acc += L.dims[v] * L.dims[v];
+    need_eig = need_eig || (reg && a.lam[v] == 0.0);
+  }
+  if (kind == kAlsIpls)
+    CCAB_CUDA(cudaMemcpyAsync(a.colmean, params + 2 * L.n_views, sizeof(double) * L.D, cudaMemcpyHostToDevice, stream));
 
   const size_t nn = (size_t)L.D * L.D;
   als_scale_copy<<<(unsigned)std::min<size_t>(ceil_div(nn, 256), 4 * (size_t)sms), 256, 0, stream>>>(G, Gw, nn,
@@ -480,8 +675,30 @@ int als_fit(int kind, const ColumnLayout& L, const double* G, double g_scale, do
   int launches = 1;
   for (int d = 0; d < k; ++d) {
     a.d = d;
+    // lam == 0 views of the regression kinds: the eigendecomposition of this dimension's G_ii (synchronises the stream)
+    for (int v = 0; need_eig && v < L.n_views; ++v) {
+      if (a.lam[v] != 0.0) continue;
+      JacobiArgs<double> ja;
+      memset(&ja, 0, sizeof(ja));
+      ja.in = Gw + (size_t)L.coff[v] * L.D + L.coff[v];
+      ja.ld_in = L.D;
+      ja.batch_stride_in = 0;
+      ja.colmajor_in = 1;  // symmetric
+      ja.m = ja.n = L.dims[v];
+      ja.batch = 1;
+      ja.out_vals = ev + L.coff[v];
+      ja.vals_stride = L.dims[v];
+      ja.out_right = V + a.voff[v];
+      ja.ld_right = L.dims[v];
+      ja.right_stride = (int64_t)L.dims[v] * L.dims[v];
+      int info = 0;
+      ja.info = &info;
+      const int rc = jacobi_solve<double>(ja, reinterpret_cast<void*>(base + o.jac), o.total - o.jac, stream);
+      if (rc) return rc;
+      CCAB_CHECK_ARG(info > 0, "the eigensolver of view %d did not converge (dimension %d)", v, d);
+    }
     void* args[] = {&a};
-    CCAB_CUDA(cudaLaunchCooperativeKernel((const void*)als_dimension, dim3(per_sm * sms), dim3(kThreads), args, smem,
+    CCAB_CUDA(cudaLaunchCooperativeKernel(kern, dim3(per_sm * sms), dim3(threads), args, smem,
                                           stream));
     ++launches;
     if (d + 1 < k) {

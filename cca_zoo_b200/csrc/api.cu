@@ -3,6 +3,7 @@
 #include "../../include/ccab200.h"
 
 #include <cstdarg>
+#include <cmath>
 #include <cstring>
 #include <atomic>
 #include <exception>
@@ -590,14 +591,20 @@ int ccab_mcca_fit(int dtype, int n_views, const int64_t* dims, const double* mom
 size_t ccab_als_fit_workspace_bytes(int n_views, const int64_t* dims) {
   ColumnLayout L;
   if (!dims || n_views < 2 || make_layout(n_views, dims, &L)) return 0;
-  return als_fit_workspace_bytes(L);
+  return als_fit_workspace_bytes(L, false);
+}
+
+size_t ccab_als_regression_workspace_bytes(int n_views, const int64_t* dims) {
+  ColumnLayout L;
+  if (!dims || n_views < 2 || make_layout(n_views, dims, &L)) return 0;
+  return als_fit_workspace_bytes(L, true);
 }
 
 int ccab_als_fit(int kind, int n_views, const int64_t* dims, const double* G, double g_scale, double n_samples,
                  const double* params, double mu, const double* init, int k, int max_iter, double tol, double* W_out,
                  int* iters_out, void* workspace, size_t workspace_bytes, void* stream) {
   CCAB_TRY
-  CCAB_CHECK_ARG(kind >= CCAB_ALS_PLS && kind <= CCAB_ALS_ADMM, "bad ALS kind %d", kind);
+  CCAB_CHECK_ARG(kind >= CCAB_ALS_PLS && kind <= CCAB_ALS_IPLS, "bad ALS kind %d", kind);
   CCAB_CHECK_ARG(n_views >= 2, "the ALS estimators need at least 2 views, got %d", n_views);
   CCAB_CHECK_ARG(dims && G && init && W_out && iters_out && workspace, "null pointer argument");
   CCAB_CHECK_ARG(kind == CCAB_ALS_PLS || params, "params is NULL");
@@ -606,7 +613,18 @@ int ccab_als_fit(int kind, int n_views, const int64_t* dims, const double* G, do
   ColumnLayout L;
   int rc = make_layout(n_views, dims, &L);
   if (rc) return rc;
-  for (int v = 0; kind != CCAB_ALS_PLS && v < n_views; ++v) {
+  const bool reg = kind == CCAB_ALS_ELASTIC || kind == CCAB_ALS_IPLS;
+  for (int v = 0; reg && v < n_views; ++v) {
+    const double alpha = params[2 * v], l1 = params[2 * v + 1];
+    CCAB_CHECK_ARG(alpha >= 0.0 && alpha < INFINITY, "alpha[%d] = %g is not a finite non-negative number", v, alpha);
+    CCAB_CHECK_ARG(l1 >= 0.0 && l1 <= 1.0, "l1_ratio[%d] = %g is not in [0, 1]", v, l1);
+    CCAB_CHECK_ARG(dims[v] <= 2048, "view %d has %lld features; ElasticCCA / SCCA_IPLS take at most 2048 per view", v,
+                   (long long)dims[v]);
+  }
+  CCAB_CHECK_ARG(!reg || n_samples > 0.0, "ElasticCCA / SCCA_IPLS need n_samples > 0");
+  CCAB_CHECK_ARG(!reg || (mu >= 0.0 && mu < 1.0), "the eigenvalue cut mu = %g of ElasticCCA / SCCA_IPLS is not in [0, 1)",
+                 mu);
+  for (int v = 0; kind != CCAB_ALS_PLS && !reg && v < n_views; ++v) {
     CCAB_CHECK_ARG(params[v] >= 0.0, "params[%d] = %g is negative", v, params[v]);
     CCAB_CHECK_ARG(kind != CCAB_ALS_SPAN || (params[v] >= 1.0 && params[v] == (double)(int64_t)params[v]),
                    "span[%d] = %g is not a positive integer", v, params[v]);

@@ -579,14 +579,33 @@ def decode_fit_block(host: torch.Tensor, offsets, dims, k: int, dtype):
     return hdr, mean, sig, ws
 
 
-ALS_KINDS = {"pls": 0, "pmd": 1, "parkhomenko": 2, "span": 3, "admm": 4}
+def column_means(mom: torch.Tensor, dims, n_total: float):
+    """Column means of the views (float64 numpy, hstack order) from the column sums that follow the padded Dp x Dp
+    moment matrix in a moments buffer (each view padded to a multiple of 128 columns, see ccab_moments_size)."""
+    import numpy as np
+
+    pads = [(int(p) + 127) // 128 * 128 for p in dims]
+    Dp = sum(pads)
+    sums = mom[Dp * Dp:Dp * Dp + Dp].to(torch.float64).cpu().numpy()
+    off = np.concatenate([[0], np.cumsum(pads)]).astype(int)
+    return np.concatenate([sums[off[i]:off[i] + int(p)] for i, p in enumerate(dims)]) / float(n_total)
 
 
-def als_fit(cov, dims, n_total, kind: str, params, init, max_iter: int, tol: float, mu: float = 1.0):
+ALS_KINDS = {"pls": 0, "pmd": 1, "parkhomenko": 2, "span": 3, "admm": 4, "elastic": 5, "ipls": 6}
+
+
+ALS_RCOND_F64 = 1e-12   # relative eigenvalue cut of the alpha l1 = 0 regressions on an exact (float64) Gram matrix
+
+
+def als_fit(cov, dims, n_total, kind: str, params, init, max_iter: int, tol: float, mu: float | None = None):
     """Sparse / ALS fit on the block covariance (ccab_als_fit): ``cov`` is the float64 D x D covariance on the device,
     the iteration runs on the Gram matrix (n_total - 1) cov.  ``init`` (k x D float64, host or device) holds the
-    initial weights of every dimension.  Returns (W (D x k float64 numpy), sweeps per dimension) after ONE copy to the
-    host."""
+    initial weights of every dimension.  ``params``: one value per view, or for "elastic" / "ipls" the pairs
+    (alpha_i, l1_ratio_i) flattened, followed for "ipls" by the D column means of the views (zeros when centred).
+    ``mu``: the ADMM penalty (default 1), or for "elastic" / "ipls" the relative eigenvalue cut of the alpha l1 = 0
+    solves (default ALS_RCOND_F64).  Returns (W (D x k float64 numpy), sweeps per dimension) after ONE copy to the
+    host; a dimension in which a coordinate descent stopped at its sweep limit above the KKT bound is reported by a
+    ConvergenceWarning, as sklearn's solvers do."""
     import numpy as np
 
     lib = _lib.load()
@@ -598,15 +617,33 @@ def als_fit(cov, dims, n_total, kind: str, params, init, max_iter: int, tol: flo
     d = _lib.i64_array(dims)
     init = torch.as_tensor(init, dtype=torch.float64).to(cov.device).contiguous()
     out = torch.empty(D * k + (k + 1) // 2, dtype=torch.float64, device=cov.device)   # W | int32 sweeps[k]
-    ws = _ws(lib.ccab_als_fit_workspace_bytes(len(dims), d), cov.device)
-    pp = (C.c_double * len(dims))(*[float(x) for x in params])
+    regression = kind in ("elastic", "ipls")
+    if mu is None:
+        mu = ALS_RCOND_F64 if regression else 1.0
+    ws_bytes = (lib.ccab_als_regression_workspace_bytes if regression else lib.ccab_als_fit_workspace_bytes)(len(dims), d)
+    ws = _ws(ws_bytes, cov.device)
+    if regression:
+        want = 2 * len(dims) + (D if kind == "ipls" else 0)
+        if len(params) != want:
+            raise ValueError(f"als_fit({kind!r}) takes {want} params, got {len(params)}")
+    pp = (C.c_double * max(len(params), len(dims)))(*[float(x) for x in params])
     with torch.cuda.device(cov.device):
         rc = lib.ccab_als_fit(ALS_KINDS[kind], len(dims), d, _ptr(cov), float(n_total - 1), float(n_total), pp,
                               float(mu), _ptr(init), k, int(max_iter), float(tol), _ptr(out),
                               C.c_void_p(out.data_ptr() + 8 * D * k), _ptr(ws), ws.numel(), _stream(cov))
     _lib.check(rc, "ccab_als_fit")
     host = out.cpu().numpy()
-    return host[:D * k].reshape(D, k).copy(), host[D * k:].view(np.int32)[:k].astype(int).tolist()
+    iters = host[D * k:].view(np.int32)[:k].astype(int).tolist()
+    capped = [d for d, it in enumerate(iters) if it < 0]
+    if capped:
+        import warnings
+
+        from sklearn.exceptions import ConvergenceWarning
+
+        warnings.warn(f"als_fit({kind!r}): a coordinate descent of latent dimension(s) {capped} stopped at its sweep "
+                      "limit above the KKT bound (1e-12 max(1, ||b||_inf)); consider a larger alpha",
+                      ConvergenceWarning, stacklevel=2)
+    return host[:D * k].reshape(D, k).copy(), [abs(it) for it in iters]
 
 
 EY_HEADER = 8      # doubles in front of W and the velocity in the state block of ccab_ey_fit

@@ -260,10 +260,23 @@ int ccab_mcca_fit(int dtype, int n_views, const int64_t* dims, const double* mom
  *   kind       CCAB_ALS_*
  *   params     per-view (host, n_views doubles): PMD tau (L1 bound tau * sqrt(d_i)), Parkhomenko / ADMM tau, Span span
  *              (1 <= span); ignored (may be NULL) for PLS_ALS
- *   mu         ADMM penalty; n_samples: the ADMM step 1 / (||G_ii||_F / n_samples + mu)
+ *              ElasticCCA / SCCA_IPLS: 2 * n_views doubles (alpha_i >= 0, l1_ratio_i in [0, 1]) per view; SCCA_IPLS
+ *              then D more: the column means of the views (zeros when they are centred)
+ *   mu         ADMM penalty; n_samples: the ADMM step 1 / (||G_ii||_F / n_samples + mu), the n of the regressions.
+ *              ElasticCCA / SCCA_IPLS: mu in [0, 1) is the relative eigenvalue cut of the alpha l1 = 0 solve
+ *              (eigenvalues of G_ii / n + rho at or below mu times the largest count as zero)
  *   init       device, k x D: the initial weights of each dimension (unit norm per view)
  *   W_out      device, D x k row-major (hstack of the views' weights);  iters_out: device int[k], sweeps per dimension
+ *              (ElasticCCA / SCCA_IPLS: negated when a coordinate descent of that dimension stopped at its 1000 sweeps
+ *              above the KKT bound)
  * Needs 2 <= n_views <= 8; the widest view must fit the shared memory of one CTA (up to ~28000 features).
+ * ElasticCCA and SCCA_IPLS solve each view update as the penalised regression of sklearn's Ridge / Lasso / ElasticNet
+ * on the Gram matrix, min 1/2 w^T (G_ii / n + rho I) w - b^T w + alpha l1 ||w||_1 (rho = alpha (1 - l1), Ridge:
+ * alpha / n_samples), to a KKT residual of 1e-12 max(1, ||b||_inf): the minimum-norm solution through an
+ * eigendecomposition of G_ii per dimension when alpha l1 = 0 (this synchronises the stream once per eigensolver
+ * sweep, so those calls are not asynchronous), cyclic coordinate descent otherwise (at most 1000 sweeps, the max_iter
+ * of sklearn's solvers).  Views of at most 2048 features; their workspace is ccab_als_regression_workspace_bytes
+ * (ccab_als_fit_workspace_bytes is that of kinds 0-4).
  * Replaces cca_zoo/linear/_iterative.py:65-117 (fit / _fit_single with the _update_weight of each model) and
  * deflate (cca_zoo/_utils/_linalg.py:91-116). */
 #define CCAB_ALS_PLS 0
@@ -271,7 +284,10 @@ int ccab_mcca_fit(int dtype, int n_views, const int64_t* dims, const double* mom
 #define CCAB_ALS_PARKHOMENKO 2
 #define CCAB_ALS_SPAN 3
 #define CCAB_ALS_ADMM 4
+#define CCAB_ALS_ELASTIC 5
+#define CCAB_ALS_IPLS 6
 size_t ccab_als_fit_workspace_bytes(int n_views, const int64_t* dims);
+size_t ccab_als_regression_workspace_bytes(int n_views, const int64_t* dims);
 int ccab_als_fit(int kind, int n_views, const int64_t* dims, const double* G, double g_scale, double n_samples,
                  const double* params, double mu, const double* init, int k, int max_iter, double tol, double* W_out,
                  int* iters_out, void* workspace, size_t workspace_bytes, void* stream);

@@ -1,6 +1,8 @@
 """Benchmark of the sparse / ALS path: SCCA_PMD(tau=0.3, latent_dimensions=4) on n = 1e5 samples of two 1024-wide
 float32 views that live in HBM.  Prints one JSON line per tolerance: tol = 0 (a fixed max_iter = 500 sweeps per
-dimension) and the default tol = 1e-6.
+dimension) and the default tol = 1e-6.  Then one line each for ElasticCCA(alpha=0.01, l1_ratio=0.5),
+SCCA_IPLS(alpha=0.01) and SCCA_IPLS() (alpha = 0: the eigendecomposition route) at the default tol: fit_ms and
+ms_per_view_update = fit_ms / (2 x the sweeps of all dimensions), which includes the moment pass and the eigensolves.
 
     python tools/bench_sparse.py [--reps 10] [--warmup 3] [--no-cpu-baseline]
 
@@ -107,6 +109,27 @@ def main():
             line["cpu_baseline"] = ("oracle.sparse.ref_als_fit (reference algorithm in data space, numpy, "
                                     "this host's CPUs)")
             line["cpu_baseline_sweeps"] = it_cpu
+        print(json.dumps(line), flush=True)
+
+    # ElasticCCA / SCCA_IPLS: the regression kinds, default tol
+    from cca_zoo_b200.linear import SCCA_IPLS, ElasticCCA
+
+    for est in (ElasticCCA(alpha=0.01, l1_ratio=0.5, latent_dimensions=k, random_state=0),
+                SCCA_IPLS(alpha=0.01, l1_ratio=1.0, latent_dimensions=k, random_state=0),
+                SCCA_IPLS(latent_dimensions=k, random_state=0)):
+        fit_ms = []
+        for r in range(args.warmup + args.reps):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            est.fit(views)
+            torch.cuda.synchronize()
+            if r >= args.warmup:
+                fit_ms.append(1e3 * (time.perf_counter() - t0))
+        iters = est._fit_info["iters"]
+        fm = statistics.median(fit_ms)
+        line = {"workload": f"{type(est).__name__}(alpha={est.alpha}, l1_ratio={est.l1_ratio}, k=4) n=1e5 "
+                            "d=[1024,1024] fp32 in HBM", "tol": est.tol, "fit_ms": round(fm, 3), "sweeps": iters,
+                "ms_per_view_update": round(fm / (2 * sum(iters)), 3), "gpu": name, "power_limit": power}
         print(json.dumps(line), flush=True)
 
 
