@@ -357,10 +357,10 @@ class BaseModel(BaseEstimator, ABC):
         validated = validate_views(self._as_numpy_views(views))
         return [(v - m) @ w for v, m, w in zip(validated, self.means_, self.weights_)]
 
-    def _transform_device(self, validated):
+    def _transform_device(self, validated, weights=None):
         device = self._device()
         out = []
-        for v, m, w in zip(validated, self.means_, self.weights_):
+        for v, m, w in zip(validated, self.means_, self.weights_ if weights is None else weights):
             X = self._to_device(v, device)
             np_dt = np.result_type(X.cpu().numpy().dtype if False else (np.float32 if X.dtype == torch.float32
                                                                          else np.float64), w.dtype)

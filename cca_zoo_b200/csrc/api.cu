@@ -12,6 +12,7 @@
 #include "ccaloss.cuh"
 #include "cholinv.cuh"
 #include "common.cuh"
+#include "gfa.cuh"
 #include "dense.cuh"
 #include "ey.cuh"
 #include "fit.cuh"
@@ -677,6 +678,31 @@ int ccab_ey_fit(int n_views, const int64_t* dims, int k, double c, double learni
   p.momentum = momentum;
   p.tol = tol;
   return ey_fit(L, p, cov, dtype, views, ld, idx, state, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+  CCAB_CATCH
+}
+
+size_t ccab_gfa_fit_workspace_bytes(int n_views, const int64_t* dims, int k) {
+  ColumnLayout L;
+  if (!dims || n_views < 1 || k < 1 || k > kGfaMaxK || make_layout(n_views, dims, &L)) return 0;
+  return gfa_fit_workspace_bytes(L, k);
+}
+
+int ccab_gfa_fit(int n_views, const int64_t* dims, int k, const double* G, double n_samples, const double* XtZ0,
+                 double tol, int drop_k, int n_steps, double* state, void* workspace, size_t workspace_bytes,
+                 void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(n_views >= 1, "GFA needs at least 1 view, got %d", n_views);
+  CCAB_CHECK_ARG(dims && G && XtZ0 && state && workspace, "null pointer argument");
+  CCAB_CHECK_ARG(k >= 1 && k <= kGfaMaxK, "k = %d: the GFA fit supports 1 <= k <= %d", k, kGfaMaxK);
+  CCAB_CHECK_ARG(n_steps >= 0, "bad n_steps %d", n_steps);
+  CCAB_CHECK_ARG(n_samples > 0.0, "n_samples = %g is not positive", n_samples);
+  ColumnLayout L;
+  int rc = make_layout(n_views, dims, &L);
+  if (rc) return rc;
+  rc = require_device();
+  if (rc) return rc;
+  return gfa_fit(L, k, G, n_samples, XtZ0, tol, drop_k, n_steps, state, workspace, workspace_bytes,
+                 static_cast<cudaStream_t>(stream));
   CCAB_CATCH
 }
 

@@ -720,6 +720,124 @@ def ey_fit(dims, init, c, learning_rate, momentum, tol, cov=None, views=None, ba
     return EyFit(dims, init, c, learning_rate, momentum, tol, cov=cov, views=views, batch=batch)
 
 
+GFA_MAX_K = 64
+GFA_HEADER = 16    # doubles of counters in front of the state block of ccab_gfa_fit
+_GFA_SLOTS = 8     # per-view arrays of the state block have this many slots (_lib.MAX_VIEWS)
+GFA_ARD_ALPHA_0 = GFA_ARD_BETA_0 = GFA_TAU_ALPHA_0 = GFA_TAU_BETA_0 = 1e-14   # CCAGFA::getDefaultOpts() priors
+GFA_INIT_TAU = 1e3
+
+
+def gfa_layout(K: int, D: int) -> dict:
+    """Offsets (doubles) of the arrays in the state block of ccab_gfa_fit (include/ccab200.h), and its ``total``."""
+    V, o, at = _GFA_SLOTS, {}, GFA_HEADER
+    for name, size in (("y_const", V), ("a_ard", V), ("a_tau", V), ("tau", V), ("b_tau", V), ("alpha", V * K),
+                       ("b_ard", V * K), ("cov_w", V * K * K), ("ww", V * K * K), ("cov_z", K * K), ("zz", K * K),
+                       ("index", K), ("W", K * D), ("B0", K * D), ("B1", K * D), ("GB0", K * D), ("GB1", K * D)):
+        o[name] = at
+        at += size
+    o["total"] = at
+    return o
+
+
+class GfaFit:
+    """One GFA fit on the device (ccab_gfa_fit): the state block and the workspace, kept across chunked calls.
+
+    ``G`` is the float64 D x D Gram matrix (CUDA), ``XtZ0`` the D x k float64 product X^T z0 (CUDA).  The host writes
+    the initial state once: tau = 1e3, alpha_m = k d_m / max(datavar_m - 1e-3, 1e-8) from the (always centred) data
+    variance of each view, zz = z0^T z0 + n I, and the constants y_const_m = tr G_mm.  ``run(n)`` enqueues one call of
+    up to n iterations; ``stopped()`` reads the stop flag back (one small copy); ``result()`` copies the state block to
+    the host once and returns it decoded (dictionary of numpy arrays at the active width k)."""
+
+    def __init__(self, dims, G, n_samples, XtZ0, z0tz0, datavar, y_const, tol, drop_k=True):
+        import numpy as np
+
+        self.lib = _lib.load()
+        self.dims = [int(d) for d in dims]
+        m, D = len(self.dims), int(sum(self.dims))
+        self.D, self.k = D, int(XtZ0.shape[1])
+        _require_cuda(G, "G")
+        _require_cuda(XtZ0, "XtZ0")
+        if G.dtype != torch.float64 or tuple(G.shape) != (D, D):
+            raise ValueError(f"G must be the float64 {D} x {D} Gram matrix")
+        if XtZ0.dtype != torch.float64 or tuple(XtZ0.shape) != (D, self.k):
+            raise ValueError(f"XtZ0 must be a float64 {D} x k matrix")
+        self.device = G.device
+        self._d = _lib.i64_array(self.dims)
+        nbytes = self.lib.ccab_gfa_fit_workspace_bytes(m, self._d, self.k)
+        if nbytes == 0:
+            raise ValueError(f"ccab_gfa_fit does not support widths {self.dims} with k = {self.k} (1 <= k <= "
+                             f"{GFA_MAX_K}, 1 to {_lib.MAX_VIEWS} views)")
+        self.G = G.contiguous()
+        self.XtZ0 = XtZ0.T.contiguous()                   # k x D: column x of X^T z0 is row x
+        self.n, self.tol, self.drop_k = float(n_samples), float(tol), bool(drop_k)
+        self.ws = _ws(nbytes, self.device)
+        K, o = self.k, gfa_layout(self.k, D)
+        self.o = o
+        h = np.zeros(o["total"])
+        h[1] = K
+        d = np.asarray(self.dims, dtype=np.float64)
+        h[o["y_const"]:o["y_const"] + m] = y_const
+        h[o["a_ard"]:o["a_ard"] + m] = GFA_ARD_ALPHA_0 + d / 2.0
+        h[o["a_tau"]:o["a_tau"] + m] = GFA_TAU_ALPHA_0 + self.n * d / 2.0
+        h[o["tau"]:o["tau"] + m] = GFA_INIT_TAU
+        h[o["b_tau"]:o["b_tau"] + m] = GFA_TAU_BETA_0
+        alpha = h[o["alpha"]:o["alpha"] + _GFA_SLOTS * K].reshape(_GFA_SLOTS, K)
+        for i in range(m):
+            alpha[i] = K * self.dims[i] / max(float(datavar[i]) - 1.0 / GFA_INIT_TAU, 1e-8)
+        h[o["b_ard"]:o["b_ard"] + _GFA_SLOTS * K] = GFA_ARD_BETA_0
+        h[o["cov_z"]:o["cov_z"] + K * K] = np.eye(K).reshape(-1)
+        h[o["zz"]:o["zz"] + K * K] = (np.asarray(z0tz0, dtype=np.float64) + self.n * np.eye(K)).reshape(-1)
+        h[o["index"]:o["index"] + K] = np.arange(K)
+        self.state = torch.from_numpy(h).to(self.device)
+        self._flag = torch.empty(1, dtype=torch.float64, pin_memory=True)
+
+    def run(self, n_steps: int):
+        with torch.cuda.device(self.device):
+            rc = self.lib.ccab_gfa_fit(len(self.dims), self._d, self.k, _ptr(self.G), self.n, _ptr(self.XtZ0), self.tol,
+                                       int(self.drop_k), int(n_steps), _ptr(self.state), _ptr(self.ws), self.ws.numel(),
+                                       C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        _lib.check(rc, "ccab_gfa_fit")
+
+    def stopped(self) -> bool:
+        self._flag.copy_(self.state[3:4])
+        return bool(self._flag[0] != 0.0)
+
+    def result(self) -> dict:
+        return decode_gfa_state(self.state.cpu().numpy(), self.dims, self.k)
+
+
+def decode_gfa_state(h, dims, K: int) -> dict:
+    """The state block of ccab_gfa_fit (host float64 array) as numpy arrays at the active width k: counters, tau,
+    b_tau, alpha / b_ard (m x k), cov_w / ww (m x k x k), cov_z, zz, index, and W, B, GB, B_prev, GB_prev (D x k)."""
+    import numpy as np
+
+    m, D = len(dims), int(sum(dims))
+    o = gfa_layout(K, D)
+    k = int(h[1])
+    cur = int(h[4])
+
+    def kk(at, count=None):
+        blk = h[at:at + (count or 1) * K * K].reshape(count or 1, K, K)[:, :k, :k].copy()
+        return blk if count else blk[0]
+
+    def kd(at):
+        return h[at:at + K * D].reshape(K, D)[:k].T.copy()
+
+    B, GB = (o["B0"], o["B1"]), (o["GB0"], o["GB1"])
+    return dict(iters=int(h[0]), k=k, stable=int(h[2]), stop=bool(h[3]), rel=float(h[5]), prunes=int(h[6]),
+                tau=h[o["tau"]:o["tau"] + m].copy(), b_tau=h[o["b_tau"]:o["b_tau"] + m].copy(),
+                alpha=h[o["alpha"]:o["alpha"] + m * K].reshape(m, K)[:, :k].copy(),
+                b_ard=h[o["b_ard"]:o["b_ard"] + m * K].reshape(m, K)[:, :k].copy(),
+                cov_w=kk(o["cov_w"], m), ww=kk(o["ww"], m), cov_z=kk(o["cov_z"]), zz=kk(o["zz"]),
+                index=h[o["index"]:o["index"] + k].astype(np.int64), W=kd(o["W"]), B=kd(B[cur]), GB=kd(GB[cur]),
+                B_prev=kd(B[cur ^ 1]), GB_prev=kd(GB[cur ^ 1]))
+
+
+def gfa_fit(dims, G, n_samples, XtZ0, z0tz0, datavar, y_const, tol, drop_k=True) -> GfaFit:
+    """The device state of one GFA fit (see ``GfaFit``)."""
+    return GfaFit(dims, G, n_samples, XtZ0, z0tz0, datavar, y_const, tol, drop_k=drop_k)
+
+
 def column_sums(view):
     """Column sums of an (n, d) CUDA tensor as one GEMM with a row of ones (float64 result)."""
     ones = torch.ones((1, view.shape[0]), dtype=view.dtype, device=view.device)

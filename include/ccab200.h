@@ -315,6 +315,36 @@ int ccab_ey_fit(int n_views, const int64_t* dims, int k, double c, double learni
                 int n_steps, const double* cov, int dtype, const void* const* views, const int64_t* ld, int batch,
                 const int32_t* idx, double* state, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- GFA (Group Factor Analysis) behind the ABI ----------------------------------------------------------------------
+ * Up to n_steps iterations of the closed-form mean-field variational loop, iterated on the Gram matrix: from the first
+ * Z update on the latent mean is z = X B, B = [tau_1 W_1; ...; tau_m W_m] cov_z, so each iteration costs one D x D x k
+ * product G B whatever n is.  ALL iterations run in one persistent cooperative launch, asynchronous, no host
+ * synchronisation; float64 throughout, fixed-order reductions only (repeated calls give bit-identical results, and any
+ * split of the iterations into calls gives the same state bit for bit).
+ *   G          the float64 Gram matrix X^T X of the hstacked views (centred when the fit centres), D x D, row-major,
+ *              symmetric (the kernel reads its rows as columns)
+ *   n_samples  n (the zz = z^T z + n cov_z term and the pruning statistic mean(z^2, 0) = diag(B^T G B) / n)
+ *   XtZ0       X^T z0 stored transposed (k x D row-major: XtZ0[x * D + r]), z0 the random start; read by the first
+ *              iteration only
+ *   tol        relative change of z below which an iteration counts as quiet; 1000 quiet iterations in a row, with no
+ *              pruning, set the stop flag, after which later iterations and later calls do nothing
+ *   drop_k     non-zero: columns whose mean(z^2) is not above 1e-7 are pruned (unless all are), compacting every
+ *              array of the state in place in index order
+ * The caller-owned state block (doubles; K = k the capacity, D = sum(dims), 8 slots per per-view array):
+ *   [0] iterations done  [1] active columns k'  [2] quiet iterations in a row  [3] stop flag  [4] parity (which of
+ *   the B / GB pairs is current)  [5] relative change of the last iteration (NaN when not compared)  [6] prunes
+ *   [7..15] reserved; then y_const[8] (tr G_mm), a_ard[8], a_tau[8], tau[8], b_tau[8], alpha[8][K], b_ard[8][K],
+ *   cov_w[8][K][K], ww[8][K][K], cov_z[K][K], zz[K][K], index[K] (original column of each active one), W[K][D],
+ *   B[2][K][D], GB[2][K][D].  Matrices keep leading dimension K; column x of W, B, GB is the row x * D .. x * D + D.
+ *   The caller initialises it (header zero, k' = K; the constants; tau = 1e3; b_tau, b_ard = 1e-14; alpha from the
+ *   data variance; zz = z0^T z0 + n I; index = 0..K-1).
+ * Needs 1 <= n_views <= 8 and 1 <= k <= 64 (workspace_bytes returns 0 otherwise).
+ * Replaces the loop of GFA.fit, cca_zoo/probabilistic/_gfa.py:217-286. */
+size_t ccab_gfa_fit_workspace_bytes(int n_views, const int64_t* dims, int k);
+int ccab_gfa_fit(int n_views, const int64_t* dims, int k, const double* G, double n_samples, const double* XtZ0,
+                 double tol, int drop_k, int n_steps, double* state, void* workspace, size_t workspace_bytes,
+                 void* stream);
+
 /* ---- the deep-CCA objective behind the ABI (any widths) ---------------------------------------------------------
  * ccab_ccaloss_fwd: loss[0] = -|| S11^-1/2 S12 S22^-1/2 ||_F^2 with S_ii = cov(z_i) + eps I, from the moment pass over
  * [z1 z2] (precision as in ccab_moments), a batched Cholesky + inverse and 7 GEMMs; `saved`
