@@ -1,6 +1,7 @@
 """cca_zoo_b200 -- H100-native drop-in for the covariance -> eigensolve hot path of cca_zoo.
 
-``cca_zoo_b200.linear`` mirrors ``cca_zoo.linear`` (CCA, rCCA, PLS, MCCA, GCCA, PartialCCA, GRCCA) and
+``cca_zoo_b200.linear`` mirrors ``cca_zoo.linear`` (CCA, rCCA, PLS, MCCA, GCCA, PartialCCA, GRCCA, the iterative,
+gradient and tensor (TCCA) estimators) and
 ``cca_zoo_b200.deep.objectives`` mirrors ``cca_zoo.deep.objectives`` (CCALoss, MCCALoss, GCCALoss) and
 ``cca_zoo_b200.probabilistic`` provides ``GFA`` of ``cca_zoo.probabilistic``.
 All arithmetic runs in hand-written sm_90a kernels (libccab200.so, include/ccab200.h).

@@ -19,6 +19,7 @@
 #include "moments.cuh"
 #include "syevj.cuh"
 #include "syevj_small.cuh"
+#include "tcca.cuh"
 #include "tgemm.cuh"
 
 namespace ccab {
@@ -678,6 +679,58 @@ int ccab_ey_fit(int n_views, const int64_t* dims, int k, double c, double learni
   p.momentum = momentum;
   p.tol = tol;
   return ey_fit(L, p, cov, dtype, views, ld, idx, state, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+  CCAB_CATCH
+}
+
+size_t ccab_tcca_moment_workspace_bytes(int n_views, const int64_t* dims, int64_t n, int nsplit) {
+  if (tcca_check_dims(n_views, dims) || n < 1) return 0;
+  return tcca_moment_workspace_bytes(n_views, dims, n, nsplit);
+}
+
+int ccab_tcca_moment(int n_views, const int64_t* dims, int64_t n, const double* const* Z, const int64_t* ldz,
+                     double scale, int nsplit, double* M, void* workspace, size_t workspace_bytes, void* stream) {
+  CCAB_TRY
+  int rc = tcca_check_dims(n_views, dims);
+  if (rc) return rc;
+  CCAB_CHECK_ARG(n >= 1, "krprod_moment needs at least one sample, got n = %lld", (long long)n);
+  CCAB_CHECK_ARG(Z && ldz && M, "null pointer argument");
+  for (int i = 0; i < n_views; ++i)
+    CCAB_CHECK_ARG(Z[i] && ldz[i] >= dims[i], "view %d: null pointer or leading dimension %lld < width %lld", i,
+                   (long long)ldz[i], (long long)dims[i]);
+  rc = require_device();
+  if (rc) return rc;
+  return tcca_moment(n_views, dims, n, Z, ldz, scale, nsplit, M, workspace, workspace_bytes,
+                     static_cast<cudaStream_t>(stream));
+  CCAB_CATCH
+}
+
+int64_t ccab_tcca_state_size(int n_views, const int64_t* dims, int k) {
+  if (tcca_check_dims(n_views, dims)) return -1;
+  if (k < 1 || k > kTccaMaxK) {
+    set_error("k = %d: the TCCA fit supports 1 <= k <= %d", k, kTccaMaxK);
+    return -1;
+  }
+  return (int64_t)tcca_state_doubles(n_views, dims, k);
+}
+
+size_t ccab_tcca_fit_workspace_bytes(int n_views, const int64_t* dims, int k) {
+  if (tcca_check_dims(n_views, dims) || k < 1 || k > kTccaMaxK) return 0;
+  return tcca_fit_workspace_bytes(n_views, dims, k);
+}
+
+int ccab_tcca_fit(int n_views, const int64_t* dims, int k, const double* M, const double* const* evecs,
+                  const double* lam0, const double* rand, int start, int n_iter, double* state, void* workspace,
+                  size_t workspace_bytes, void* stream) {
+  CCAB_TRY
+  int rc = tcca_check_dims(n_views, dims);
+  if (rc) return rc;
+  CCAB_CHECK_ARG(k >= 1 && k <= kTccaMaxK, "k = %d: the TCCA fit supports 1 <= k <= %d", k, kTccaMaxK);
+  CCAB_CHECK_ARG(n_iter >= 0, "bad n_iter %d", n_iter);
+  CCAB_CHECK_ARG(M && state && (!start || evecs), "null pointer argument");
+  rc = require_device();
+  if (rc) return rc;
+  return tcca_fit(n_views, dims, k, M, evecs, lam0, rand, start, n_iter, state, workspace, workspace_bytes,
+                  static_cast<cudaStream_t>(stream));
   CCAB_CATCH
 }
 

@@ -754,8 +754,11 @@ int jacobi_solve(const JacobiArgs<T>& a, void* ws, size_t ws_bytes, cudaStream_t
   const T tol = a.tol > 0 ? (T)a.tol : (T)(4.0 * (double)Eps<T>::v * std::sqrt((double)m));
   // the same cap for both precisions: the block sweeps spend a phase that grows with n before the quadratic one sets in
   // (a float32 n = 2700 SPD matrix with eigenvalues spread over [0.01, 1] converges in its 17th sweep, to eigenvalue
-  // errors of 0.005 n eps ||A||), and the cap only costs time on a solve that would otherwise be reported unconverged
-  const int max_sweeps = a.max_sweeps > 0 ? a.max_sweeps : 24;
+  // errors of 0.005 n eps ||A||), and the cap only costs time on a solve that would otherwise be reported unconverged.
+  // Rank-deficient blocks have a long phase of their own: the columns of the null cluster keep normalised
+  // off-diagonals near 1 until their norms fall below the noise floor, then the sweep converges at once (a 300 x 300
+  // float64 covariance of rank 150, 900 samples: 25 sweeps), so the cap leaves room well beyond that
+  const int max_sweeps = a.max_sweeps > 0 ? a.max_sweeps : 64;
   // fused cluster path: smallest cluster (<= 8 CTAs) whose row slice fits comfortably in shared memory; when none
   // fits (large m), each round runs as three kernels (gram / solve / apply)
   int cs = 0, rows_g = 0, rows_v = 0;

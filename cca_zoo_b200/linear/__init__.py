@@ -4,8 +4,10 @@ from ._mcca import MCCA
 from ._gcca import GCCA
 from ._partialcca import PartialCCA
 from ._grcca import GRCCA
+from ._tcca import TCCA
 from ._iterative import PLS_ALS, SCCA_ADMM, SCCA_IPLS, SCCA_PMD, ElasticCCA, ParkhomenkoCCA, SCCA_Span
 from .gradient import CCA_EY, MCCA_EY, PLS_EY
 
 __all__ = ["CCA", "rCCA", "PLS", "MCCA", "GCCA", "PartialCCA", "GRCCA", "PLS_ALS", "SCCA_PMD", "ParkhomenkoCCA",
-           "SCCA_Span", "SCCA_ADMM", "SCCA_IPLS", "ElasticCCA", "PLS_EY", "CCA_EY", "MCCA_EY"]
+           "SCCA_Span", "SCCA_ADMM", "SCCA_IPLS", "ElasticCCA", "PLS_EY", "CCA_EY", "MCCA_EY",
+           "TCCA"]

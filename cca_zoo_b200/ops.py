@@ -838,6 +838,108 @@ def gfa_fit(dims, G, n_samples, XtZ0, z0tz0, datavar, y_const, tol, drop_k=True)
     return GfaFit(dims, G, n_samples, XtZ0, z0tz0, datavar, y_const, tol, drop_k=drop_k)
 
 
+TCCA_MAX_K = 64
+TCCA_MAX_VIEWS = 8
+TCCA_MAX_ENTRIES = 1 << 25     # prod of the view widths: M in float64 is 256 MB
+TCCA_MAX_ITER = 100            # tensorly's n_iter_max
+TCCA_HEADER = 8                # doubles in front of the rec history in the state block of ccab_tcca_fit
+
+
+def tcca_moment(Z, nsplit: int = 0):
+    """M = Z_1^T KR(Z_2, ..., Z_m) / n (p_1 x prod_{i>1} p_i float64, CUDA): the mode-0 unfolding of the cross-moment
+    tensor of the float64 (n, p_i) CUDA tensors ``Z`` (ccab_tcca_moment).  ``nsplit`` > 0 forces that many sample
+    splits; 0 lets the library choose from the shape."""
+    lib = _lib.load()
+    for i, z in enumerate(Z):
+        _require_cuda(z, f"Z[{i}]")
+    Z = [_row_major(z, False) for z in Z]
+    if any(z.dtype != torch.float64 for z in Z):
+        raise ValueError("tcca_moment takes float64 views")
+    n = int(Z[0].shape[0])
+    if any(int(z.shape[0]) != n for z in Z):
+        raise ValueError("tcca_moment: the views differ in their number of rows")
+    dims = [int(z.shape[1]) for z in Z]
+    d = _lib.i64_array(dims)
+    P = 1
+    for p in dims[1:]:
+        P *= p
+    M = torch.empty((dims[0], P), dtype=torch.float64, device=Z[0].device)
+    ws = _ws(lib.ccab_tcca_moment_workspace_bytes(len(dims), d, n, int(nsplit)), M.device)
+    ptrs = (C.c_void_p * len(Z))(*[z.data_ptr() for z in Z])
+    with torch.cuda.device(M.device):
+        rc = lib.ccab_tcca_moment(len(dims), d, n, ptrs, _lib.i64_array([z.stride(0) for z in Z]), 1.0 / max(n, 1),
+                                  int(nsplit), _ptr(M), _ptr(ws), ws.numel(), _stream(M))
+    _lib.check(rc, "ccab_tcca_moment")
+    return M
+
+
+def tcca_layout(dims, k: int) -> dict:
+    """Offsets (doubles) of the state block of ccab_tcca_fit: ``rec``, ``F`` (one per mode), ``G`` and ``total``."""
+    at = TCCA_HEADER + TCCA_MAX_ITER
+    F = []
+    for p in dims:
+        F.append(at)
+        at += int(p) * k
+    return {"rec": TCCA_HEADER, "F": F, "G": at, "total": at + len(dims) * k * k}
+
+
+def tcca_fit(M, dims, k: int, n_iter: int, rand=None, state=None):
+    """CP-ALS on the tensor M (float64 CUDA, prod(dims) entries in C order) with ccab_tcca_fit; returns the device
+    state block.  Without ``state`` the fit starts: the leading eigenvectors of every unfolding Gram M_(j) M_(j)^T
+    (one DMMA GEMM and one ``syevj`` per mode) and the host-drawn random columns ``rand`` (a list, one p_j x (k - p_j)
+    array or None per mode) seed it.  With ``state`` the fit continues from it.  Up to ``n_iter`` iterations either
+    way, nothing read back."""
+    import numpy as np
+
+    lib = _lib.load()
+    _require_cuda(M, "M")
+    dims = [int(p) for p in dims]
+    m, d = len(dims), _lib.i64_array(dims)
+    total = lib.ccab_tcca_state_size(m, d, int(k))
+    if total < 0:
+        raise ValueError(f"ccab_tcca_fit: {_lib.last_error()}")
+    if M.dtype != torch.float64 or M.numel() != int(np.prod(dims)):
+        raise ValueError(f"M must be a float64 tensor of {int(np.prod(dims))} entries")
+    M = M.contiguous()
+    dev = M.device
+    ws = _ws(lib.ccab_tcca_fit_workspace_bytes(m, d, int(k)), dev)
+    keep = []
+    evecs, lam0, rnd = None, None, None
+    if state is None:
+        state = torch.empty(total, dtype=torch.float64, device=dev)
+        T = M.reshape(dims)
+        vecs = []
+        for j in range(m):
+            A = T.movedim(j, 0).reshape(dims[j], -1)
+            lam, evt = syevj(gemm(A, A, transb=True))
+            vecs.append(evt.contiguous())
+            if j == 0:
+                lam0 = lam
+        keep += vecs
+        evecs = (C.c_void_p * m)(*[v.data_ptr() for v in vecs])
+        blocks = [np.asarray(r, dtype=np.float64).reshape(-1) for r in (rand or []) if r is not None]
+        if blocks:
+            rnd = torch.from_numpy(np.concatenate(blocks)).to(dev)
+    elif state.dtype != torch.float64 or state.numel() != total or not state.is_cuda:
+        raise ValueError(f"state must be a float64 CUDA tensor of {total} elements")
+    with torch.cuda.device(dev):
+        rc = lib.ccab_tcca_fit(m, d, int(k), _ptr(M), evecs, _ptr(lam0), _ptr(rnd), int(evecs is not None),
+                               int(n_iter), _ptr(state), _ptr(ws), ws.numel(), _stream(M))
+    _lib.check(rc, "ccab_tcca_fit")
+    return state
+
+
+def decode_tcca_state(h, dims, k: int) -> dict:
+    """The state block of ccab_tcca_fit (host float64 array): iters, stop, singular, norm, rec (one per iteration
+    done), F (p_j x k per mode) and G (their Grams)."""
+    o = tcca_layout(dims, k)
+    it = int(h[0])
+    return dict(iters=it, stop=bool(h[1]), singular=bool(h[2]), norm=float(h[3]),
+                rec=h[o["rec"]:o["rec"] + it].copy(),
+                F=[h[f:f + int(p) * k].reshape(int(p), k).copy() for f, p in zip(o["F"], dims)],
+                G=h[o["G"]:o["total"]].reshape(len(dims), k, k).copy())
+
+
 def column_sums(view):
     """Column sums of an (n, d) CUDA tensor as one GEMM with a row of ones (float64 result)."""
     ones = torch.ones((1, view.shape[0]), dtype=view.dtype, device=view.device)

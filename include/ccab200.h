@@ -345,6 +345,42 @@ int ccab_gfa_fit(int n_views, const int64_t* dims, int k, const double* G, doubl
                  double tol, int drop_k, int n_steps, double* state, void* workspace, size_t workspace_bytes,
                  void* stream);
 
+/* ---- TCCA (tensor CCA) behind the ABI ---------------------------------------------------------------------------------
+ * ccab_tcca_moment: M = scale * Z_1^T KR(Z_2, ..., Z_m), the mode-0 unfolding (p_1 x prod_{i>1} p_i, row-major) of
+ * the cross-moment tensor of the whitened views.  KR is the row-wise Khatri-Rao product flattened in C order (the
+ * last view's index fastest), so M reshaped to p_1 x ... x p_m is the tensor itself.  Z[i] are float64 n x p_i
+ * row-major device matrices with leading dimension ldz[i] >= p_i.  One contraction over the samples on the fp64 tensor
+ * pipe (DMMA); the Khatri-Rao operand is generated in shared memory and never stored.  nsplit <= 0 picks the number of
+ * sample splits from the shape (splits when the output tiles cannot fill the GPU); the partial slabs are added in a
+ * fixed order, no atomics, so repeated calls are bit-identical.  workspace_bytes (0 when unsplit) sizes the slabs.
+ * Needs 2 <= n_views <= 8, every p_i >= 1, prod p_i <= 2^25, n >= 1.
+ * Replaces the n x p_1 x ... x p_m outer-product array of TCCA.fit, cca_zoo/linear/_tcca.py:99-109. */
+size_t ccab_tcca_moment_workspace_bytes(int n_views, const int64_t* dims, int64_t n, int nsplit);
+int ccab_tcca_moment(int n_views, const int64_t* dims, int64_t n, const double* const* Z, const int64_t* ldz,
+                     double scale, int nsplit, double* M, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ccab_tcca_fit: up to n_iter iterations of tensorly's parafac ALS (unnormalised, exact solve per mode, stop when
+ * |rec_prev - rec| < 1e-8 from the second iteration on, at most 100 iterations in all) on the tensor M (float64,
+ * prod p_i entries in C order), asynchronous: a fixed launch sequence in which every kernel returns at once once the
+ * stop flag is set, fixed-order reductions only (repeated calls are bit-identical).
+ * start != 0 first writes the start state from the leading eigenvectors of the unfolding Grams M_(j) M_(j)^T:
+ *   evecs[j]   p_j x p_j row-major device matrix whose row r is the eigenvector of the r-th largest eigenvalue
+ *   lam0       the eigenvalues of mode 0 (descending, device): column r of mode 0 is scaled by sqrt(max(lam0[r], 0))
+ *   rand       (device) the random start columns of every mode with p_j < k, p_j x (k - p_j) row-major each, in mode
+ *              order (tensorly draws them with one RandomState in that order); may be NULL when there are none
+ *   Column r < min(k, p_j) is eigenvector r with its entry of largest |value| (the first on ties) made positive.
+ * State block (doubles, size ccab_tcca_state_size): [0] iterations done [1] stop flag [2] singular (an exactly zero
+ * pivot in the solve of some mode, where numpy.linalg.solve raises; it also sets the stop flag) [3] ||M||_F
+ * [4..7] zero; rec[100] (the reconstruction error of every iteration); the factors F_j (p_j x k row-major) in mode
+ * order; their Grams F_j^T F_j (k x k each).
+ * Needs 2 <= n_views <= 8, 1 <= k <= 64, prod p_i <= 2^25 (state_size returns -1, workspace_bytes 0 otherwise).
+ * Replaces tensorly.decomposition.parafac(M, k, random_state=...) of TCCA.fit, cca_zoo/linear/_tcca.py:111-117. */
+int64_t ccab_tcca_state_size(int n_views, const int64_t* dims, int k);
+size_t ccab_tcca_fit_workspace_bytes(int n_views, const int64_t* dims, int k);
+int ccab_tcca_fit(int n_views, const int64_t* dims, int k, const double* M, const double* const* evecs,
+                  const double* lam0, const double* rand, int start, int n_iter, double* state, void* workspace,
+                  size_t workspace_bytes, void* stream);
+
 /* ---- the deep-CCA objective behind the ABI (any widths) ---------------------------------------------------------
  * ccab_ccaloss_fwd: loss[0] = -|| S11^-1/2 S12 S22^-1/2 ||_F^2 with S_ii = cov(z_i) + eps I, from the moment pass over
  * [z1 z2] (precision as in ccab_moments), a batched Cholesky + inverse and 7 GEMMs; `saved`
