@@ -15,6 +15,9 @@ LIB_PATH = os.path.join(_HERE, "libccab200.so")
 F32, F64 = 0, 1
 PREC_TF32, PREC_TF32X3, PREC_EXACT, PREC_TF32X3B = 0, 1, 2, 3
 MAX_VIEWS = 8
+# metric ids of ccab_pairwise_kernel (CCAB_KERNEL_* in include/ccab200.h)
+KERNEL_METRICS = {"linear": 0, "poly": 1, "polynomial": 1, "rbf": 2, "sigmoid": 3, "cosine": 4, "laplacian": 5,
+                  "chi2": 6, "additive_chi2": 7}
 
 _i64p = C.POINTER(C.c_int64)
 _vp = C.c_void_p
@@ -87,6 +90,9 @@ SIGNATURES = {
     "ccab_tcca_fit_workspace_bytes": (C.c_size_t, [C.c_int, _i64p, C.c_int]),
     "ccab_tcca_fit": (C.c_int, [C.c_int, _i64p, C.c_int, _vp, C.POINTER(_vp), _vp, _vp, C.c_int, C.c_int, _vp, _vp,
                                 C.c_size_t, _vp]),
+    "ccab_pairwise_kernel_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64]),
+    "ccab_pairwise_kernel": (C.c_int, [C.c_int, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int,
+                                       C.c_double, C.c_double, C.c_double, _vp, C.c_int64, _vp, C.c_size_t, _vp]),
     "ccab_scale": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int64,
                              _vp]),
     "ccab_center_columns": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp]),

@@ -13,6 +13,7 @@
 #include "cholinv.cuh"
 #include "common.cuh"
 #include "gfa.cuh"
+#include "kcca.cuh"
 #include "dense.cuh"
 #include "ey.cuh"
 #include "fit.cuh"
@@ -731,6 +732,32 @@ int ccab_tcca_fit(int n_views, const int64_t* dims, int k, const double* M, cons
   if (rc) return rc;
   return tcca_fit(n_views, dims, k, M, evecs, lam0, rand, start, n_iter, state, workspace, workspace_bytes,
                   static_cast<cudaStream_t>(stream));
+  CCAB_CATCH
+}
+
+size_t ccab_pairwise_kernel_workspace_bytes(int metric, int64_t nx, int64_t ny) {
+  if (metric < CCAB_KERNEL_LINEAR || metric > CCAB_KERNEL_ADDITIVE_CHI2 || nx < 0 || ny < 0) return 0;
+  return pairwise_kernel_workspace_bytes(metric, nx, ny);
+}
+
+int ccab_pairwise_kernel(int metric, int dtype, const void* X, int64_t nx, int64_t ldx, const void* Y, int64_t ny,
+                         int64_t ldy, int d, double gamma, double degree, double coef0, double* K, int64_t ldk,
+                         void* workspace, size_t workspace_bytes, void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(metric >= CCAB_KERNEL_LINEAR && metric <= CCAB_KERNEL_ADDITIVE_CHI2, "bad kernel metric %d", metric);
+  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
+  CCAB_CHECK_ARG(nx >= 0 && ny >= 0 && d >= 1, "bad shape nx=%lld ny=%lld d=%d", (long long)nx, (long long)ny, d);
+  CCAB_CHECK_ARG(ldx >= d && ldy >= d && ldk >= ny, "leading dimension too small");
+  CCAB_CHECK_ARG(nx <= ((int64_t)1 << 31) && ny <= ((int64_t)1 << 31), "pairwise_kernel: more than 2^31 rows");
+  CCAB_CHECK_ARG((X && Y && K) || nx == 0 || ny == 0, "null pointer argument");
+  int rc = require_device();
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (dtype == CCAB_F32)
+    return pairwise_kernel<float>(metric, static_cast<const float*>(X), nx, ldx, static_cast<const float*>(Y), ny,
+                                  ldy, d, gamma, degree, coef0, K, ldk, workspace, workspace_bytes, s);
+  return pairwise_kernel<double>(metric, static_cast<const double*>(X), nx, ldx, static_cast<const double*>(Y), ny,
+                                 ldy, d, gamma, degree, coef0, K, ldk, workspace, workspace_bytes, s);
   CCAB_CATCH
 }
 

@@ -984,3 +984,44 @@ def frobenius_norm(A):
         rc = lib.ccab_frobenius_norm(_DT[A.dtype], A.shape[0], A.shape[1], _ptr(A), A.stride(0), _ptr(out), _stream(A))
     _lib.check(rc, "ccab_frobenius_norm")
     return out
+
+
+def pairwise_kernel(X, Y=None, metric: str = "linear", gamma: float = 1.0, degree: float = 1.0, coef0: float = 1.0):
+    """K = k(X, Y) (float64, n_x x n_y, CUDA) for a metric name of sklearn's PAIRWISE_KERNEL_FUNCTIONS
+    (ccab_pairwise_kernel).  X, Y: 2-D float32 / float64 CUDA tensors with unit column stride (any leading dimension)
+    and one dtype; Y None means X (then, as in sklearn, the rbf distance is exactly 0 on the diagonal).  ``gamma`` is
+    the resolved value (the caller applies sklearn's default 1 / n_features).  chi2 / additive_chi2 raise sklearn's
+    ValueError on negative input, which costs one scalar read-back."""
+    lib = _lib.load()
+    if metric not in _lib.KERNEL_METRICS:
+        raise ValueError(f"unknown kernel {metric!r}: supported are {sorted(_lib.KERNEL_METRICS)}")
+    _require_cuda(X, "X")
+    X = _row_major(X, False)
+    Y = X if Y is None else _row_major(Y, False)
+    _require_cuda(Y, "Y")
+    if X.dtype != Y.dtype or X.dtype not in _DT or X.device != Y.device:
+        raise ValueError(f"pairwise_kernel: X and Y must share one float dtype and device, got {X.dtype}@{X.device} "
+                         f"and {Y.dtype}@{Y.device}")
+    if X.shape[1] != Y.shape[1]:
+        raise ValueError(f"Incompatible dimension for X and Y matrices: X.shape[1] == {X.shape[1]} while "
+                         f"Y.shape[1] == {Y.shape[1]}")
+    if metric in ("chi2", "additive_chi2"):
+        neg = bool(((X < 0).any() | (Y < 0).any()).item())
+        if neg:
+            raise ValueError("X contains negative values." if bool((X < 0).any().item())
+                             else "Y contains negative values.")
+    met = _lib.KERNEL_METRICS[metric]
+    nx, ny, d = int(X.shape[0]), int(Y.shape[0]), int(X.shape[1])
+    K = torch.empty((nx, ny), dtype=torch.float64, device=X.device)
+    ws = _ws(lib.ccab_pairwise_kernel_workspace_bytes(met, nx, ny), X.device)
+    with torch.cuda.device(X.device):
+        rc = lib.ccab_pairwise_kernel(met, _DT[X.dtype], _ptr(X), nx, X.stride(0), _ptr(Y), ny, Y.stride(0), d,
+                                      float(gamma), float(degree), float(coef0), _ptr(K), ny, _ptr(ws), ws.numel(),
+                                      _stream(X))
+    _lib.check(rc, "ccab_pairwise_kernel")
+    return K
+
+
+KCCA_MAX_VIEWS = 8
+KCCA_MAX_SAMPLES = 8192
+KCCA_MAX_ORDER = 16384     # m * n: the whitened matrix T is at most 16384^2 float64 = 2 GB

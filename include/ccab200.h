@@ -381,6 +381,37 @@ int ccab_tcca_fit(int n_views, const int64_t* dims, int k, const double* M, cons
                   const double* lam0, const double* rand, int start, int n_iter, double* state, void* workspace,
                   size_t workspace_bytes, void* stream);
 
+/* ---- KCCA: pairwise kernel matrices ------------------------------------------------------------------------------
+ * ccab_pairwise_kernel: K = k(X, Y) (nx x ny float64, row-major, ldk) for the metric names of sklearn's
+ * PAIRWISE_KERNEL_FUNCTIONS, computed as sklearn.metrics.pairwise_kernels does:
+ *   LINEAR         x.y
+ *   POLY           (gamma x.y + coef0)^degree                     (pow with a float degree)
+ *   RBF            exp(-gamma max(|x|^2 + |y|^2 - 2 x.y, 0))      (0 distance on the diagonal when X is Y)
+ *   SIGMOID        tanh(gamma x.y + coef0)
+ *   COSINE         x.y / (|x| |y|)                                (0 for a zero row)
+ *   LAPLACIAN      exp(-gamma sum_k |x_k - y_k|)
+ *   CHI2           exp(-gamma sum_k (x_k - y_k)^2 / (x_k + y_k))  (terms with x_k + y_k = 0 skipped)
+ *   ADDITIVE_CHI2  -sum_k (x_k - y_k)^2 / (x_k + y_k)
+ * X (nx x d, ldx) and Y (ny x d, ldy) are row-major device matrices in `dtype` (float32 is widened to float64 on
+ * load); "X is Y" means the same pointer, row count and leading dimension.  The inner-product metrics run on the fp64
+ * tensor pipe (DMMA) with the metric fused into the epilogue, after a row-norm pre-pass for RBF / COSINE; the
+ * distance metrics run as FMA tiles.  Every element is summed over the features in one fixed order: repeated calls
+ * are bit-identical.  CHI2 / ADDITIVE_CHI2 need non-negative input, which the caller checks (sklearn raises).
+ * workspace_bytes: (nx + ny) doubles for RBF / COSINE, 0 otherwise.
+ * Replaces sklearn.metrics.pairwise_kernels of KCCA.fit / KCCA.transform, cca_zoo/nonparametric/_kcca.py:137-183. */
+#define CCAB_KERNEL_LINEAR 0
+#define CCAB_KERNEL_POLY 1
+#define CCAB_KERNEL_RBF 2
+#define CCAB_KERNEL_SIGMOID 3
+#define CCAB_KERNEL_COSINE 4
+#define CCAB_KERNEL_LAPLACIAN 5
+#define CCAB_KERNEL_CHI2 6
+#define CCAB_KERNEL_ADDITIVE_CHI2 7
+size_t ccab_pairwise_kernel_workspace_bytes(int metric, int64_t nx, int64_t ny);
+int ccab_pairwise_kernel(int metric, int dtype, const void* X, int64_t nx, int64_t ldx, const void* Y, int64_t ny,
+                         int64_t ldy, int d, double gamma, double degree, double coef0, double* K, int64_t ldk,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- the deep-CCA objective behind the ABI (any widths) ---------------------------------------------------------
  * ccab_ccaloss_fwd: loss[0] = -|| S11^-1/2 S12 S22^-1/2 ||_F^2 with S_ii = cov(z_i) + eps I, from the moment pass over
  * [z1 z2] (precision as in ccab_moments), a batched Cholesky + inverse and 7 GEMMs; `saved`
