@@ -120,16 +120,95 @@ def top_eigenvectors(T):
     return Yt, sweeps
 
 
-class KCCA(BaseModel):
+class _KernelModel(BaseModel):
+    """The part KCCA, KGCCA and KTCCA share: the fit preamble (parameters, limits, per-view kernel arguments, the
+    device upload, centring) and the kernel-space methods (``transform`` and ``pairwise_correlations`` evaluate the
+    kernel against ``train_views_``).  ``partial_fit`` and the sharded fit are refused: every kernel matrix needs all
+    the rows."""
+
+    _solve_in_float64 = True
+    _parameter_constraints: ClassVar[dict[str, list[Any]]] = dict(BaseModel._parameter_constraints)   # none of its own
+
+    def _check_limits(self, m: int, n: int):
+        raise NotImplementedError
+
+    def _setup_kernel_fit(self, views, extra=()):
+        """Validate, upload and centre the views; set ``means_``, ``train_views_``, ``n_views_``, ``n_features_in_``,
+        ``n_samples_`` and the resolved kernel arguments.  ``extra`` names further per-view parameters as (name,
+        value, default).  Returns (float64 device views, per-view c, the per-view ``extra`` lists, device).  Every
+        parameter and limit error is raised before anything is uploaded."""
+        self._validate_params()
+        if parallel.is_distributed():
+            raise NotImplementedError(f"{type(self).__name__} has no sharded fit: every kernel matrix needs all the rows")
+        validated = validate_views(views)
+        m, n = len(validated), int(validated[0].shape[0])
+        dims = [int(v.shape[1]) for v in validated]
+        self._check_limits(m, n)
+        c_ = [float(x) for x in perview_parameter("c", self.c, 0.1, m)]
+        kernel_ = perview_parameter("kernel", self.kernel, "linear", m)
+        gamma_ = perview_parameter("gamma", self.gamma, None, m)
+        degree_ = perview_parameter("degree", self.degree, 1.0, m)
+        coef0_ = perview_parameter("coef0", self.coef0, 1.0, m)
+        kp_ = perview_parameter("kernel_params", self.kernel_params, {}, m)
+        args = [kernel_arguments(kernel_[i], gamma_[i], degree_[i], coef0_[i], kp_[i], dims[i]) for i in range(m)]
+        extra_ = [perview_parameter(name, value, default, m) for name, value, default in extra]
+        device = self._device()
+
+        X = [self._to_device(v, device).to(torch.float64) for v in validated]
+        if any(isinstance(v, torch.Tensor) for v in validated):
+            if not bool(torch.stack([torch.isfinite(x).all() for x in X]).all().item()):
+                raise ValueError("Input contains NaN or infinity.")
+        if self.center:
+            mu = [ops.column_sums(x) / n for x in X]
+            X = [x - u.view(1, -1) for x, u in zip(X, mu)]
+            means = torch.cat(mu).cpu().numpy()
+            off = np.concatenate([[0], np.cumsum(dims)]).astype(int)
+            self.means_ = [means[off[i]:off[i + 1]].copy() for i in range(m)]
+        else:
+            X = [x.clone() for x in X]                  # train_views_ never aliases the caller's tensors
+            self.means_ = [np.zeros(p) for p in dims]
+        self.n_views_, self.n_features_in_, self.n_samples_ = m, dims, n
+        self.train_views_ = X
+        self._kernel_args = args
+        return X, c_, extra_, device
+
+    # ------------------------------------------------------------------ kernel transform
+    def transform(self, views):
+        """k_i(train_views_i, X_i)^T weights_i per view; the new views are not centred (as in the reference)."""
+        check_is_fitted(self)
+        validated = validate_views(views)
+        device = self.train_views_[0].device
+        out = []
+        for i, v in enumerate(validated):
+            Xt = self._to_device(v, device).to(torch.float64)
+            Kt = ops.pairwise_kernel(self.train_views_[i], Xt, *self._kernel_args[i])     # n_train x n_test
+            W = torch.from_numpy(np.ascontiguousarray(self.weights_[i])).to(device)
+            out.append(ops.gemm(Kt, W, transa=True).cpu().numpy())
+        return out
+
+    def pairwise_correlations(self, views):
+        """(n_views, n_views, k) Pearson correlations of the kernel variates (cca_zoo/_base.py:153-174)."""
+        T = np.stack(self.transform(views), axis=0)
+        T = T - T.mean(axis=1, keepdims=True)
+        norms = np.sqrt((T**2).sum(axis=1, keepdims=True))
+        T_norm = T / np.where(norms > 1e-12, norms, 1.0)
+        return np.einsum("isd,jsd->ijd", T_norm, T_norm)
+
+    def partial_fit(self, views, y=None, solve: bool = True):
+        raise NotImplementedError(f"{type(self).__name__} has no partial_fit: every kernel matrix needs all the rows")
+
+    def _solve(self, C, dims, n_total):
+        raise NotImplementedError(f"{type(self).__name__} solves its kernel eigenproblem in fit, not from a block "
+                                  "covariance")
+
+
+class KCCA(_KernelModel):
     r"""Kernel CCA (cca_zoo/nonparametric/_kcca.py), solved in the eigenbasis of each kernel matrix.
 
     Same arguments, defaults and fitted attributes as the reference (``weights_`` -- float64 n x k per view --,
     ``train_views_`` -- the centred float64 training views, kept on the device --, ``means_``, ``n_views_``,
     ``n_features_in_``, ``n_samples_``), plus ``device``.  Kernels: the metric names of sklearn's
     ``PAIRWISE_KERNEL_FUNCTIONS``.  Limits: at most 8 views, n <= 8192 and m n <= 16384."""
-
-    _solve_in_float64 = True
-    _parameter_constraints: ClassVar[dict[str, list[Any]]] = dict(BaseModel._parameter_constraints)   # none of its own
 
     def __init__(self, latent_dimensions: int = 1, center: bool = True, c=0.1, kernel="linear", gamma=None,
                  degree=1.0, coef0=1.0, kernel_params=None, eps: float = 1e-3, device=None) -> None:
@@ -156,41 +235,11 @@ class KCCA(BaseModel):
 
     # ------------------------------------------------------------------ fit
     def fit(self, views, y=None):
-        self._validate_params()
-        if parallel.is_distributed():
-            raise NotImplementedError("KCCA has no sharded fit: every kernel matrix needs all the rows")
-        validated = validate_views(views)
-        m, n = len(validated), int(validated[0].shape[0])
-        dims = [int(v.shape[1]) for v in validated]
-        self._check_limits(m, n)
-        c_ = [float(x) for x in perview_parameter("c", self.c, 0.1, m)]
-        kernel_ = perview_parameter("kernel", self.kernel, "linear", m)
-        gamma_ = perview_parameter("gamma", self.gamma, None, m)
-        degree_ = perview_parameter("degree", self.degree, 1.0, m)
-        coef0_ = perview_parameter("coef0", self.coef0, 1.0, m)
-        kp_ = perview_parameter("kernel_params", self.kernel_params, {}, m)
-        args = [kernel_arguments(kernel_[i], gamma_[i], degree_[i], coef0_[i], kp_[i], dims[i]) for i in range(m)]
+        X, c_, _, device = self._setup_kernel_fit(views)
+        m, n = self.n_views_, self.n_samples_
         k = min(int(self.latent_dimensions), m * n)
-        device = self._device()
 
-        X = [self._to_device(v, device).to(torch.float64) for v in validated]
-        if any(isinstance(v, torch.Tensor) for v in validated):
-            if not bool(torch.stack([torch.isfinite(x).all() for x in X]).all().item()):
-                raise ValueError("Input contains NaN or infinity.")
-        if self.center:
-            mu = [ops.column_sums(x) / n for x in X]
-            X = [x - u.view(1, -1) for x, u in zip(X, mu)]
-            means = torch.cat(mu).cpu().numpy()
-            off = np.concatenate([[0], np.cumsum(dims)]).astype(int)
-            self.means_ = [means[off[i]:off[i + 1]].copy() for i in range(m)]
-        else:
-            X = [x.clone() for x in X]                  # train_views_ never aliases the caller's tensors
-            self.means_ = [np.zeros(p) for p in dims]
-        self.n_views_, self.n_features_in_, self.n_samples_ = m, dims, n
-        self.train_views_ = X
-        self._kernel_args = args
-
-        K, knorm = kernel_matrices(X, args)
+        K, knorm = kernel_matrices(X, self._kernel_args)
         lams, U, sweeps = eigenbases(K, knorm)
         del K
         lam_h = torch.cat(lams).cpu().numpy()
@@ -217,31 +266,3 @@ class KCCA(BaseModel):
         self.weights_ = [Wh[i * n:(i + 1) * n].copy() for i in range(m)]
         self._fit_info = {"kernel_sweeps": sweeps, "sweeps": top_sweeps, "ranks": r}
         return self
-
-    # ------------------------------------------------------------------ kernel transform
-    def transform(self, views):
-        """k_i(train_views_i, X_i)^T weights_i per view; the new views are not centred (as in the reference)."""
-        check_is_fitted(self)
-        validated = validate_views(views)
-        device = self.train_views_[0].device
-        out = []
-        for i, v in enumerate(validated):
-            Xt = self._to_device(v, device).to(torch.float64)
-            Kt = ops.pairwise_kernel(self.train_views_[i], Xt, *self._kernel_args[i])     # n_train x n_test
-            W = torch.from_numpy(np.ascontiguousarray(self.weights_[i])).to(device)
-            out.append(ops.gemm(Kt, W, transa=True).cpu().numpy())
-        return out
-
-    def pairwise_correlations(self, views):
-        """(n_views, n_views, k) Pearson correlations of the kernel variates (cca_zoo/_base.py:153-174)."""
-        T = np.stack(self.transform(views), axis=0)
-        T = T - T.mean(axis=1, keepdims=True)
-        norms = np.sqrt((T**2).sum(axis=1, keepdims=True))
-        T_norm = T / np.where(norms > 1e-12, norms, 1.0)
-        return np.einsum("isd,jsd->ijd", T_norm, T_norm)
-
-    def partial_fit(self, views, y=None, solve: bool = True):
-        raise NotImplementedError("KCCA has no partial_fit: every kernel matrix needs all the rows")
-
-    def _solve(self, C, dims, n_total):
-        raise NotImplementedError("KCCA solves its kernel eigenproblem in fit, not from a block covariance")
