@@ -93,6 +93,11 @@ SIGNATURES = {
     "ccab_pairwise_kernel_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64]),
     "ccab_pairwise_kernel": (C.c_int, [C.c_int, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int,
                                        C.c_double, C.c_double, C.c_double, _vp, C.c_int64, _vp, C.c_size_t, _vp]),
+    "ccab_row_norm4_sum_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "ccab_row_norm4_sum": (C.c_int, [C.c_int, C.c_int64, C.c_int, _vp, C.c_int64, _vp, _vp, _vp, C.c_size_t, _vp]),
+    "ccab_ccar3_admm_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "ccab_ccar3_admm": (C.c_int, [C.c_int, C.c_int, _vp, C.c_int64, _vp, C.c_int64, C.c_double, C.c_double, C.c_double,
+                                  C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_size_t, _vp]),
     "ccab_scale": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int64,
                              _vp]),
     "ccab_center_columns": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp]),

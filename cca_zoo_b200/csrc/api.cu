@@ -10,6 +10,7 @@
 
 #include "als.cuh"
 #include "ccaloss.cuh"
+#include "ccar3.cuh"
 #include "cholinv.cuh"
 #include "common.cuh"
 #include "gfa.cuh"
@@ -732,6 +733,49 @@ int ccab_tcca_fit(int n_views, const int64_t* dims, int k, const double* M, cons
   if (rc) return rc;
   return tcca_fit(n_views, dims, k, M, evecs, lam0, rand, start, n_iter, state, workspace, workspace_bytes,
                   static_cast<cudaStream_t>(stream));
+  CCAB_CATCH
+}
+
+size_t ccab_row_norm4_sum_workspace_bytes(int64_t n) {
+  if (n < 1) return 0;
+  return row_norm4_sum_workspace_bytes(n);
+}
+
+int ccab_row_norm4_sum(int dtype, int64_t n, int d, const void* Y, int64_t ldy, const double* mean, double* out,
+                       void* workspace, size_t workspace_bytes, void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
+  CCAB_CHECK_ARG(n >= 1 && d >= 1, "bad shape n=%lld d=%d", (long long)n, d);
+  CCAB_CHECK_ARG(ldy >= d, "leading dimension %lld < width %d", (long long)ldy, d);
+  CCAB_CHECK_ARG(Y && mean && out, "null pointer argument");
+  int rc = require_device();
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (dtype == CCAB_F32)
+    return row_norm4_sum<float>(n, d, static_cast<const float*>(Y), ldy, mean, out, workspace, workspace_bytes, s);
+  return row_norm4_sum<double>(n, d, static_cast<const double*>(Y), ldy, mean, out, workspace, workspace_bytes, s);
+  CCAB_CATCH
+}
+
+size_t ccab_ccar3_admm_workspace_bytes(int p, int q) {
+  if (p < 1 || p > kCcar3MaxP || q < 1 || q > kCcar3MaxQ) return 0;
+  return ccar3_admm_workspace_bytes(p, q);
+}
+
+int ccab_ccar3_admm(int p, int q, const double* M, int64_t ldm, const double* B0, int64_t ldb, double kappa,
+                    double rho, double tol, int max_iter, double* Z, int64_t ldz, double* U, int64_t ldu,
+                    double* info, void* workspace, size_t workspace_bytes, void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(p >= 1 && p <= kCcar3MaxP && q >= 1 && q <= kCcar3MaxQ,
+                 "ccar3_admm supports 1 <= p <= %d and 1 <= q <= %d, got p = %d, q = %d", kCcar3MaxP, kCcar3MaxQ, p, q);
+  CCAB_CHECK_ARG(max_iter >= 1, "bad max_iter %d", max_iter);
+  CCAB_CHECK_ARG(rho > 0.0 && tol > 0.0 && kappa >= 0.0, "ccar3_admm needs rho > 0, tol > 0 and kappa >= 0");
+  CCAB_CHECK_ARG(ldm >= p && ldb >= q && ldz >= q && ldu >= q, "leading dimension too small");
+  CCAB_CHECK_ARG(M && B0 && Z && U && info, "null pointer argument");
+  int rc = require_device();
+  if (rc) return rc;
+  return ccar3_admm(p, q, M, ldm, B0, ldb, kappa, rho, tol, max_iter, Z, ldz, U, ldu, info, workspace,
+                    workspace_bytes, static_cast<cudaStream_t>(stream));
   CCAB_CATCH
 }
 

@@ -1025,3 +1025,57 @@ def pairwise_kernel(X, Y=None, metric: str = "linear", gamma: float = 1.0, degre
 KCCA_MAX_VIEWS = 8
 KCCA_MAX_SAMPLES = 8192
 KCCA_MAX_ORDER = 16384     # m * n: the whitened matrix T is at most 16384^2 float64 = 2 GB
+
+
+CCAR3_MAX_P = 16384        # M = (Sx + (rho + eps) I)^-1 is p x p float64 (2 GB)
+CCAR3_MAX_Q = 512          # the ADMM kernel keeps every output row of a CTA's row block in registers
+
+
+def row_norm4_sum(Y, mean):
+    """sum_s ||y_s - mean||^4 (1-element float64 CUDA tensor) over the rows of the float32 / float64 (n, d) CUDA tensor
+    ``Y`` (any row stride), centred with the float64 device vector ``mean`` (ccab_row_norm4_sum)."""
+    lib = _lib.load()
+    _require_cuda(Y, "Y")
+    _require_cuda(mean, "mean")
+    Y = _row_major(Y, False)
+    if Y.dtype not in _DT:
+        raise ValueError("row_norm4_sum takes a float32 or float64 view")
+    n, d = int(Y.shape[0]), int(Y.shape[1])
+    mean = mean.to(torch.float64).contiguous()
+    if mean.numel() != d:
+        raise ValueError(f"mean has {mean.numel()} entries for {d} columns")
+    out = torch.empty(1, dtype=torch.float64, device=Y.device)
+    ws = _ws(lib.ccab_row_norm4_sum_workspace_bytes(n), Y.device)
+    with torch.cuda.device(Y.device):
+        rc = lib.ccab_row_norm4_sum(_DT[Y.dtype], n, d, _ptr(Y), Y.stride(0), _ptr(mean), _ptr(out), _ptr(ws),
+                                    ws.numel(), _stream(Y))
+    _lib.check(rc, "ccab_row_norm4_sum")
+    return out
+
+
+def ccar3_admm(M, B0, kappa: float, rho: float, tol: float, max_iter: int):
+    """CCAR3's row-sparse ADMM from Z = U = 0 (ccab_ccar3_admm): ``M`` (p x p) and ``B0`` (p x q) float64 CUDA
+    matrices, kappa = lambda / rho.  Returns (Z, U, info) on the device, nothing read back; info = (iterations,
+    primal, dual, stopped) as float64[4]."""
+    lib = _lib.load()
+    _require_cuda(M, "M")
+    _require_cuda(B0, "B0")
+    M, B0 = _row_major(M, False), _row_major(B0, False)
+    p, q = int(B0.shape[0]), int(B0.shape[1])
+    if M.dtype != torch.float64 or B0.dtype != torch.float64 or tuple(M.shape) != (p, p):
+        raise ValueError(f"ccar3_admm takes a float64 p x p M and p x q B0, got {tuple(M.shape)} {M.dtype} and "
+                         f"{tuple(B0.shape)} {B0.dtype}")
+    nbytes = lib.ccab_ccar3_admm_workspace_bytes(p, q)
+    if nbytes == 0:
+        raise ValueError(f"ccar3_admm supports 1 <= p <= {CCAR3_MAX_P} and 1 <= q <= {CCAR3_MAX_Q}, got p = {p}, "
+                         f"q = {q}")
+    Z = torch.empty((p, q), dtype=torch.float64, device=M.device)
+    U = torch.empty_like(Z)
+    info = torch.empty(4, dtype=torch.float64, device=M.device)
+    ws = _ws(nbytes, M.device)
+    with torch.cuda.device(M.device):
+        rc = lib.ccab_ccar3_admm(p, q, _ptr(M), M.stride(0), _ptr(B0), B0.stride(0), float(kappa), float(rho),
+                                 float(tol), int(max_iter), _ptr(Z), q, _ptr(U), q, _ptr(info), _ptr(ws), ws.numel(),
+                                 _stream(M))
+    _lib.check(rc, "ccab_ccar3_admm")
+    return Z, U, info

@@ -412,6 +412,33 @@ int ccab_pairwise_kernel(int metric, int dtype, const void* X, int64_t nx, int64
                          int64_t ldy, int d, double gamma, double degree, double coef0, double* K, int64_t ldk,
                          void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- CCAR3: reduced-rank-regression CCA -------------------------------------------------------------------------
+ * ccab_row_norm4_sum: out[0] (device double) = sum_s ||y_s - mean||^4 over the n rows of Y (n x d row-major, ldy,
+ * float32 or float64 in `dtype`), centred on the fly with mean (device double[d]); accumulated in float64 in a fixed
+ * order (one warp per row, a grid chosen from n alone, block sums added in block order): repeated calls are
+ * bit-identical.  It is the one data-dependent term of the Ledoit-Wolf shrinkage that the block moments lack.
+ * Replaces the sum of (X^2)^T X^2 inside sklearn.covariance.ledoit_wolf_shrinkage, behind
+ * LedoitWolf().fit(Y) in CCAR3.fit, cca_zoo/linear/_ccar3.py:221. */
+size_t ccab_row_norm4_sum_workspace_bytes(int64_t n);
+int ccab_row_norm4_sum(int dtype, int64_t n, int d, const void* Y, int64_t ldy, const double* mean, double* out,
+                       void* workspace, size_t workspace_bytes, void* stream);
+
+/* ccab_ccar3_admm: the row-sparse group-lasso ADMM of CCAR3 in inverse form on float64 device matrices,
+ *   B = B0 + rho M (Z - U);   Z_old = Z;   Z = row_shrink(B + U);   U = U + B - Z,
+ *   row_shrink scales each row r by max(0, 1 - kappa / ||r||) (rows of norm 0 stay 0),
+ * from Z = U = 0 (both are overwritten, p x q row-major, ldz / ldu), for up to max_iter iterations, stopping after
+ * the first iteration with max(||Z - B||_F, ||Z_old - Z||_F) / sqrt(p) < tol.  M = (Sx + (rho + eps) I)^-1 is p x p
+ * (ldm), B0 = M Sxy Sy^-1/2 is p x q (ldb), kappa = lambda / rho.  Z holds the result (exact zero rows).
+ * info (device double[4]) = iterations done, the last primal and dual residuals, and 1 if the tolerance stopped the
+ * loop (0 when max_iter did).  One persistent cooperative launch, one grid barrier per iteration, no host
+ * synchronisation; the products run on the fp64 tensor pipe (DMMA) and every sum has a fixed order, so repeated calls
+ * are bit-identical.  1 <= p <= 16384, 1 <= q <= 512; workspace_bytes is 0 outside them.
+ * Replaces _admm_row_sparse_rrr, cca_zoo/linear/_ccar3.py:37-80 (two LU solves of order p per iteration). */
+size_t ccab_ccar3_admm_workspace_bytes(int p, int q);
+int ccab_ccar3_admm(int p, int q, const double* M, int64_t ldm, const double* B0, int64_t ldb, double kappa,
+                    double rho, double tol, int max_iter, double* Z, int64_t ldz, double* U, int64_t ldu,
+                    double* info, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- the deep-CCA objective behind the ABI (any widths) ---------------------------------------------------------
  * ccab_ccaloss_fwd: loss[0] = -|| S11^-1/2 S12 S22^-1/2 ||_F^2 with S_ii = cov(z_i) + eps I, from the moment pass over
  * [z1 z2] (precision as in ccab_moments), a batched Cholesky + inverse and 7 GEMMs; `saved`
