@@ -1,7 +1,8 @@
 // K3/K4: symmetric eigensolver and SVD by one-sided block Jacobi (Hestenes), batched.
 //
 // The working matrix G (m x n, column-major: each column contiguous) starts as A (symmetric mode) or
-// as the matrix to factor (SVD mode); V (n x n) starts as I.  Columns are grouped in blocks of
+// as the matrix to factor (SVD mode), multiplied by the power of two that brings max |G| into [0.5, 1) (exact; the
+// values are scaled back at the end); V (n x n) starts as I.  Columns are grouped in blocks of
 // kB = 16.  One round of the round-robin tournament handles nb/2 disjoint block pairs; for a pair
 // the 32-column panel P = [G_p G_q] gets
 //     (a) its Gram matrix  W = P^T P                      (jacobi_gram_kernel, row-split partials)
@@ -168,6 +169,7 @@ struct JacobiCtx {
   int* skip;     // [batch][npairs]
   unsigned* stat;  // [batch] max off-diagonal ratio of the sweep (float bits)
   float* null2;    // [batch] squared column norm below which a column is numerical noise: (n eps)^2 ||G||_F^2
+  int* expo;       // [batch] G was multiplied by 2^-expo before the sweeps (max |G| in [0.5, 1))
   int m, n_pad, nb, npairs, R;
   int64_t ldg;
   int rows_per_part;
@@ -541,20 +543,47 @@ __global__ void jacobi_init_kernel(const T* __restrict__ in, int64_t ld_in, int6
   if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) c.stat[b] = 0u;
 }
 
-// null2[b] = (n eps)^2 ||G_b||_F^2 (one block per matrix, fixed-order reduction: deterministic).  n eps ||A||_F bounds the
-// rounding error of a column of A V (|fl(A v) - A v| <= n eps |A| |v|), so a column below it carries no direction.  A
-// larger floor stops refining genuine columns: at 10 n eps ||A||_F, a float32 n = 2700 SPD matrix with eigenvalues in
-// [0.01, 1] had every eigenvalue below 0.048 left unrefined (eigenvalue errors of 7.6e-3).
+// One block per matrix, fixed-order reductions (deterministic):
+//  * expo[b] = the exponent of max |G_b| (frexp), and G_b <- 2^-expo G_b, so that max |G_b| lies in [0.5, 1).  The
+//    sweeps form products of four entries (w_ii w_jj in the convergence test, a_pp a_qq and a_pq^2 in the rotation
+//    test), and the noise floor below is kept in float: away from unit scale these under- or overflow (a float64
+//    covariance of data at 1e-12, a float32 matrix with entries near 1e9), no pair gets a ratio, and the sweep
+//    reports convergence with V still the identity.  A power of two is exact, so the solve of 2^k A is the solve of A
+//    bit for bit and jacobi_values_kernel multiplies the values back by 2^expo.  A zero matrix keeps expo = 0.
+//  * null2[b] = (n eps)^2 ||G_b||_F^2 of the normalised G_b.  n eps ||A||_F bounds the rounding error of a column of
+//    A V (|fl(A v) - A v| <= n eps |A| |v|), so a column below it carries no direction.  A larger floor stops refining
+//    genuine columns: at 10 n eps ||A||_F, a float32 n = 2700 SPD matrix with eigenvalues in [0.01, 1] had every
+//    eigenvalue below 0.048 left unrefined (eigenvalue errors of 7.6e-3).
 template <typename T>
-__global__ void jacobi_scale_kernel(const JacobiCtx<T> c, int n, float* __restrict__ null2) {
+__global__ void jacobi_scale_kernel(const JacobiCtx<T> c, int n) {
   __shared__ double red[32];
+  __shared__ int expo_s;
   const int b = blockIdx.x;
-  const T* G = c.G + (size_t)b * c.n_pad * c.ldg;
-  double acc = 0.0;
+  T* G = c.G + (size_t)b * c.n_pad * c.ldg;
+  // ldg == m (make_plan): the n columns of G_b are one run of n m elements, walked without a division per element
   const size_t total = (size_t)n * c.m;
+  T amax = T(0);
+#pragma unroll 4
+  for (size_t e = threadIdx.x; e < total; e += blockDim.x) amax = fmax(amax, fabs(G[e]));
+  for (int o = 16; o > 0; o >>= 1) amax = fmax(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = (double)amax;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t = fmax(t, red[w]);
+    int ex = 0;
+    if (t > 0.0) frexp(t, &ex);
+    expo_s = ex;
+    c.expo[b] = ex;
+  }
+  __syncthreads();
+  const int ex = expo_s;
+  double acc = 0.0;
+#pragma unroll 4
   for (size_t e = threadIdx.x; e < total; e += blockDim.x) {
-    const double v = (double)G[(e / c.m) * c.ldg + (e % c.m)];
-    acc += v * v;
+    const T v = ldexp(G[e], -ex);
+    G[e] = v;
+    acc += (double)v * (double)v;
   }
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
@@ -563,7 +592,7 @@ __global__ void jacobi_scale_kernel(const JacobiCtx<T> c, int n, float* __restri
     double t = 0.0;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
     const double ne = (double)n * (double)Eps<T>::v;
-    null2[b] = (float)fmin(ne * ne * t, 3.0e38);   // norm threshold n eps ||G||_F
+    c.null2[b] = (float)fmin(ne * ne * t, 3.0e38);   // norm threshold n eps ||G||_F
   }
 }
 
@@ -571,7 +600,8 @@ __global__ void jacobi_reset_stat_kernel(unsigned* stat, int batch) {
   if (threadIdx.x < batch) stat[threadIdx.x] = 0u;
 }
 
-// one warp per column: value (Rayleigh quotient or norm), pad detection, optional normalisation of G
+// one warp per column: value (Rayleigh quotient or norm), pad detection, optional normalisation of G.  The value is
+// formed in the scale of the normalised G and multiplied back by 2^expo (exact).
 template <typename T>
 __global__ void jacobi_values_kernel(JacobiCtx<T> c, int n, int svd_mode, T shift, T* __restrict__ vals,
                                      T* __restrict__ vnorm) {
@@ -594,15 +624,18 @@ __global__ void jacobi_values_kernel(JacobiCtx<T> c, int n, int svd_mode, T shif
     padw += __shfl_xor_sync(0xffffffffu, padw, o);
     vv += __shfl_xor_sync(0xffffffffu, vv, o);
   }
+  const int ex = c.expo[b];
   T val;
   if (padw > T(0.5)) {
     val = neg_inf<T>();  // padding direction: sorts last, never output
   } else if (svd_mode) {
-    val = sqrt(acc);
-    const T inv = val > T(0) ? T(1) / val : T(0);
+    const T nrm = sqrt(acc);
+    const T inv = nrm > T(0) ? T(1) / nrm : T(0);
     for (int i = lane; i < c.m; i += 32) g[i] *= inv;
+    val = ldexp(nrm, ex);
   } else {
-    val = (vv > T(0) ? acc / vv : acc) - shift;  // Rayleigh quotient of the (re-normalised) vector
+    // Rayleigh quotient of the (re-normalised) vector, un-shifted by the shift in the same scale
+    val = ldexp((vv > T(0) ? acc / vv : acc) - ldexp(shift, -ex), ex);
   }
   if (lane == 0) {
     vals[(size_t)b * c.n_pad + col] = val;
@@ -679,7 +712,7 @@ template <typename T>
 struct Plan {
   int n_pad, nb, npairs, R, rows_per_part;
   int64_t ldg;
-  size_t oG, oV, oW, oQ, oSkip, oStat, oNull, oVals, oNorm, oRank, total;
+  size_t oG, oV, oW, oQ, oSkip, oStat, oNull, oExpo, oVals, oNorm, oRank, total;
 };
 
 template <typename T>
@@ -702,6 +735,7 @@ Plan<T> make_plan(int m, int n, int batch) {
   P.oSkip = o; o += al((size_t)batch * P.npairs * sizeof(int));
   P.oStat = o; o += al((size_t)batch * sizeof(unsigned));
   P.oNull = o; o += al((size_t)batch * sizeof(float));
+  P.oExpo = o; o += al((size_t)batch * sizeof(int));
   P.oVals = o; o += al((size_t)batch * P.n_pad * sizeof(T));
   P.oNorm = o; o += al((size_t)batch * P.n_pad * sizeof(T));
   P.oRank = o; o += al((size_t)batch * P.n_pad * sizeof(int));
@@ -732,6 +766,7 @@ int jacobi_solve(const JacobiArgs<T>& a, void* ws, size_t ws_bytes, cudaStream_t
   c.skip = reinterpret_cast<int*>(w + P.oSkip);
   c.stat = reinterpret_cast<unsigned*>(w + P.oStat);
   c.null2 = reinterpret_cast<float*>(w + P.oNull);
+  c.expo = reinterpret_cast<int*>(w + P.oExpo);
   T* vals = reinterpret_cast<T*>(w + P.oVals);
   T* vnorm = reinterpret_cast<T*>(w + P.oNorm);
   int* rank = reinterpret_cast<int*>(w + P.oRank);
@@ -748,7 +783,7 @@ int jacobi_solve(const JacobiArgs<T>& a, void* ws, size_t ws_bytes, cudaStream_t
     const int rows = std::max(m, P.n_pad);
     dim3 grid((unsigned)std::min<int64_t>(ceil_div(rows, 256), 64), P.n_pad, batch);
     jacobi_init_kernel<T><<<grid, 256, 0, stream>>>(a.in, a.ld_in, a.batch_stride_in, a.colmajor_in, m, n, c, shift); count_launches(1);
-    jacobi_scale_kernel<T><<<batch, 1024, 0, stream>>>(c, n, c.null2); count_launches(1);
+    jacobi_scale_kernel<T><<<batch, 1024, 0, stream>>>(c, n); count_launches(1);
     CCAB_CUDA(cudaGetLastError());
   }
   const T tol = a.tol > 0 ? (T)a.tol : (T)(4.0 * (double)Eps<T>::v * std::sqrt((double)m));

@@ -9,6 +9,7 @@
 // alongside.  Two block barriers per step, n - 1 steps per sweep, software-pipelined: the rotations of step t + 1 are
 // computed (by n/2 threads) while the other threads rotate the eigenvectors of step t; only the upper triangle of H
 // is kept.  The off-diagonal mass seen during a sweep decides convergence on the device.  Eigenvalues are returned in descending order with the eigenvectors as rows.
+// H is solved multiplied by the power of two that brings max |H| into [0.5, 1), and the eigenvalues are scaled back.
 //
 // Two-sided Jacobi resolves eigenvalues to eps * ||H|| (absolute): right for the Ritz problem, whose block is well
 // conditioned; the whitening eigenproblems (tiny eigenvalues matter relatively) stay on the one-sided solver of
@@ -91,28 +92,52 @@ syevj_small_kernel(const T* __restrict__ A, int64_t lda, int64_t strideA, int n,
   int* label = reinterpret_cast<int*>(rot + 2 * m2);     // [2][N] original index held by a position (-1: the bye)
   int* rank = label + 2 * N;                             // [N]
   __shared__ int done;
+  __shared__ int expo;
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
   const T* Ab = A + (size_t)blockIdx.y * strideA;
 
-  // ---- load (symmetrised), V = I (own columns), ||H||_F^2 ----
-  T fro_local = T(0);
+  // ---- load (symmetrised), V = I (own columns), max |H| ----
+  T amax = T(0);
 #pragma unroll 4
   for (int e = tid; e < N * N; e += kSmallThreads) {
     const int r = e / N, c = e % N;
     T v = T(0);
     if (r < n && c < n) v = T(0.5) * (Ab[(size_t)r * lda + c] + Ab[(size_t)c * lda + r]);
     H0[r * LD + c] = v;
-    fro_local = fma(v, v, fro_local);
+    amax = fmax(amax, fabs(v));
   }
   for (int e = tid; e < N * cw; e += kSmallThreads) {
     const int r = e / cw, c = e % cw;
     V0[r * LDV + c] = (r == c0 + c && r < n) ? T(1) : T(0);
   }
   if (tid < N) label[tid] = tid < n ? tid : -1;
-  for (int o = 16; o > 0; o >>= 1) fro_local += __shfl_xor_sync(0xffffffffu, fro_local, o);
-  if (lane == 0) red[warp] = fro_local;
+  for (int o = 16; o > 0; o >>= 1) amax = fmax(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  if (lane == 0) red[warp] = amax;
   if (tid == 0) done = 0;
+  __syncthreads();
+  // ---- H <- 2^-expo H with max |H| in [0.5, 1), ||H||_F^2 ----
+  // The rotation and convergence tests below compare sums of squares: away from unit scale they under- or overflow
+  // (a float32 matrix with entries near 1e20 makes ||H||_F^2 infinite and the first sweep "converged").  A power of
+  // two is exact, so the solve of 2^k A is the solve of A bit for bit; the eigenvalues are scaled back when written.
+  // A zero matrix keeps expo = 0.
+  {
+    for (int w = 0; w < kSmallThreads / 32; ++w) amax = fmax(amax, red[w]);
+    int ex = 0;
+    if (amax > T(0)) frexp(amax, &ex);
+    if (tid == 0) expo = ex;
+    __syncthreads();
+    T fro_local = T(0);
+#pragma unroll 4
+    for (int e = tid; e < N * N; e += kSmallThreads) {
+      const int r = e / N, c = e % N;
+      const T v = ldexp(H0[r * LD + c], -ex);
+      H0[r * LD + c] = v;
+      fro_local = fma(v, v, fro_local);
+    }
+    for (int o = 16; o > 0; o >>= 1) fro_local += __shfl_xor_sync(0xffffffffu, fro_local, o);
+    if (lane == 0) red[warp] = fro_local;
+  }
   __syncthreads();
   T fro2 = T(0);
   for (int w = 0; w < kSmallThreads / 32; ++w) fro2 += red[w];
@@ -259,7 +284,7 @@ syevj_small_kernel(const T* __restrict__ A, int64_t lda, int64_t strideA, int n,
         const T lj = H[j * LD + j];
         rk += (lj > li || (lj == li && j < tid)) ? 1 : 0;
       }
-      if (evals && blockIdx.x == 0) evals[(size_t)blockIdx.y * strideE + rk] = li;
+      if (evals && blockIdx.x == 0) evals[(size_t)blockIdx.y * strideE + rk] = ldexp(li, expo);
     }
     rank[tid] = rk;
   }
