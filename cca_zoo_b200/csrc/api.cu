@@ -834,7 +834,7 @@ int ccab_scale(int dtype, int m, int n, const void* A, int64_t lda, const void* 
                int c_pow, void* B, int64_t ldb, void* stream) {
   CCAB_TRY
   CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
-  CCAB_CHECK_ARG(A && B, "null pointer argument");
+  CCAB_CHECK_ARG((A && B) || m == 0 || n == 0, "null pointer argument");   // an empty tensor may have no storage
   CCAB_CHECK_ARG(r_pow >= 0 && r_pow <= 2 && c_pow >= 0 && c_pow <= 2, "bad power code");
   int rc = require_device();
   if (rc) return rc;
@@ -850,7 +850,7 @@ int ccab_scale(int dtype, int m, int n, const void* A, int64_t lda, const void* 
 int ccab_center_columns(int dtype, int m, int n, void* A, int64_t lda, void* stream) {
   CCAB_TRY
   CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
-  CCAB_CHECK_ARG(A != nullptr, "null pointer argument");
+  CCAB_CHECK_ARG(A != nullptr || m == 0 || n == 0, "null pointer argument");
   int rc = require_device();
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -862,7 +862,8 @@ int ccab_center_columns(int dtype, int m, int n, void* A, int64_t lda, void* str
 int ccab_frobenius_norm(int dtype, int m, int n, const void* A, int64_t lda, void* out, void* stream) {
   CCAB_TRY
   CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
-  CCAB_CHECK_ARG(A && out, "null pointer argument");
+  CCAB_CHECK_ARG(out && (A || m == 0 || n == 0), "null pointer argument");
+  CCAB_CHECK_ARG(m >= 0 && n >= 0, "bad shape");
   int rc = require_device();
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);

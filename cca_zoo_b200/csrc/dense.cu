@@ -413,25 +413,29 @@ __device__ __forceinline__ T pow_code(T v, int code) {
   return v;
 }
 
+// columns on grid.x, rows on grid.y with a grid-stride loop: gridDim.y stops at 65535, the row count does not
 template <typename T>
 __global__ void scale_kernel(int m, int n, const T* __restrict__ A, int64_t lda, const T* __restrict__ r, int r_pow,
                              const T* __restrict__ c, int c_pow, T* __restrict__ B, int64_t ldb) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  const int i = blockIdx.y;
   if (j >= n) return;
-  T f = T(1);
-  if (r) f *= pow_code(r[i], r_pow);
-  if (c) f *= pow_code(c[j], c_pow);
-  B[(size_t)i * ldb + j] = A[(size_t)i * lda + j] * f;
+  const T fc = c ? pow_code(c[j], c_pow) : T(1);
+  for (int i = blockIdx.y; i < m; i += gridDim.y) {
+    T f = T(1);
+    if (r) f *= pow_code(r[i], r_pow);
+    if (c) f *= fc;
+    B[(size_t)i * ldb + j] = A[(size_t)i * lda + j] * f;
+  }
 }
 
 template <typename T>
 int scale_rows_cols(int m, int n, const T* A, int64_t lda, const T* r, int r_pow, const T* c, int c_pow, T* B,
                     int64_t ldb, cudaStream_t stream) {
+  CCAB_CHECK_ARG(m >= 0 && n >= 0, "bad shape");
   if (m == 0 || n == 0) return 0;
-  CCAB_CHECK_ARG(m <= 65535 * 1024, "too many rows");
-  scale_kernel<T><<<dim3((unsigned)ceil_div(n, 128), (unsigned)m), 128, 0, stream>>>(m, n, A, lda, r, r_pow, c, c_pow,
-                                                                                     B, ldb); count_launches(1);
+  const unsigned rows = (unsigned)std::min(m, 65535);
+  scale_kernel<T><<<dim3((unsigned)ceil_div(n, 128), rows), 128, 0, stream>>>(m, n, A, lda, r, r_pow, c, c_pow, B,
+                                                                              ldb); count_launches(1);
   CCAB_CUDA(cudaGetLastError());
   return 0;
 }
@@ -472,13 +476,34 @@ int center_columns(int m, int n, T* A, int64_t lda, cudaStream_t stream) {
 template int center_columns<float>(int, int, float*, int64_t, cudaStream_t);
 template int center_columns<double>(int, int, double*, int64_t, cudaStream_t);
 
+// Two passes in one CTA.  Pass 1 finds max |a| and the exponent e that puts max |a| 2^-e in [0.5, 1); pass 2 sums
+// (a 2^-e)^2 in a fixed order and the norm is 2^e sqrt(sum).  The scaling is exact and moves every square by the even
+// power 2^-2e, so at ordinary scales the result is sqrt(sum a^2) bit for bit, while the squares can neither overflow
+// (entries past 2^511) nor vanish (entries below 2^-537): frob(2^k A) = 2^k frob(A) exactly over the whole range.
 template <typename T>
 __global__ void frobenius_kernel(int m, int n, const T* __restrict__ A, int64_t lda, T* __restrict__ out) {
   __shared__ double red[32];
-  double acc = 0.0;
+  __shared__ int e_s;
   const size_t total = (size_t)m * n;
+  double mx = 0.0;
+  for (size_t i = threadIdx.x; i < total; i += blockDim.x) mx = fmax(mx, fabs((double)A[(i / n) * lda + (i % n)]));
+  for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    mx = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.0;
+    for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (threadIdx.x == 0) {
+      int e = 0;                                // zero matrix: sum 0; inf: e = 0 keeps the inf
+      if (isfinite(mx) && mx > 0.0) frexp(mx, &e);
+      e_s = e;
+    }
+  }
+  __syncthreads();
+  const int e = e_s;
+  double acc = 0.0;
   for (size_t i = threadIdx.x; i < total; i += blockDim.x) {
-    const double v = (double)A[(i / n) * lda + (i % n)];
+    const double v = ldexp((double)A[(i / n) * lda + (i % n)], -e);
     acc += v * v;
   }
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -487,7 +512,7 @@ __global__ void frobenius_kernel(int m, int n, const T* __restrict__ A, int64_t 
   if (threadIdx.x < 32) {
     acc = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.0;
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if (threadIdx.x == 0) out[0] = (T)sqrt(acc);
+    if (threadIdx.x == 0) out[0] = (T)ldexp(sqrt(acc), e);
   }
 }
 
