@@ -23,7 +23,7 @@ from __future__ import annotations
 import numpy as np
 
 from .restatement import block_slices, perview, setup_fit
-from .sparse import als_init
+from .sparse import als_init, dimension_record, update_record
 
 ELASTIC_KINDS = ("elastic", "ipls")
 KKT_TOL = 1e-12
@@ -45,9 +45,11 @@ def kkt_residual(Q, b, lam, w):
     return float(r.max()) if r.size else 0.0
 
 
-def solve_penalised(Gii, b, n, alpha, l1, w0, rcond=RCOND, report=None):
+def solve_penalised(Gii, b, n, alpha, l1, w0, rcond=RCOND, report=None, rec=None):
     """argmin 1/2 w^T (Gii / n + rho I) w - b^T w + alpha l1 ||w||_1 (see the module docstring).  A coordinate
-    descent still above the KKT bound after CD_SWEEPS sweeps appends False to ``report`` (a list)."""
+    descent still above the KKT bound after CD_SWEEPS sweeps appends False to ``report`` (a list).  ``rec`` (a dict)
+    receives the eigenvalue cut with the smallest kept and the largest dropped mu_k (lam = 0), or the KKT residual
+    of every sweep of the coordinate descent and its bound (lam > 0)."""
     p = b.size
     rho, lam = (alpha / n if l1 == 0.0 else alpha * (1.0 - l1)), alpha * l1  # Ridge's alpha is not divided by n
     Q = Gii / n + rho * np.eye(p)
@@ -55,11 +57,19 @@ def solve_penalised(Gii, b, n, alpha, l1, w0, rcond=RCOND, report=None):
         ev, V = np.linalg.eigh(Gii)
         mk = ev / n + rho
         inv = np.where(mk > rcond * max(mk.max(), 0.0), 1.0 / np.where(mk > 0, mk, 1.0), 0.0)
+        if rec is not None:
+            cut = rcond * max(mk.max(), 0.0)
+            rec.update(cut=float(cut), kept_min=float(mk[mk > cut].min(initial=np.inf)),
+                       dropped_max=float(mk[mk <= cut].max(initial=-np.inf)))
         return V @ (inv * (V.T @ b))
     tol = KKT_TOL * max(1.0, float(np.abs(b).max(initial=0.0)))
     w = np.array(w0, dtype=np.float64)
+    if rec is not None:
+        rec.update(kkt_tol=tol, kkt=[])
     for sweep in range(CD_SWEEPS + 1):
         g = Q @ w - b
+        if rec is not None:
+            rec["kkt"].append(kkt_residual(Q, b, lam, w))
         if kkt_residual(Q, b, lam, w) <= tol:
             break
         if sweep == CD_SWEEPS:
@@ -76,22 +86,26 @@ def solve_penalised(Gii, b, n, alpha, l1, w0, rcond=RCOND, report=None):
     return w
 
 
-def _loop(kind, dims, w, params, n, max_iter, tol, cross, gram_ii, colmean, report):
+def _loop(kind, dims, w, params, n, max_iter, tol, cross, gram_ii, colmean, report, rcond=RCOND, trace=None):
     """One latent dimension.  ``cross(w, i)`` -> (X_i^T t, ||t||) with the model's target t (ElasticCCA: all views,
     SCCA_IPLS: the others); ``gram_ii(i)`` -> X_i^T X_i; ``colmean(i)`` -> column means of X_i.  Returns the deltas;
-    a capped coordinate descent appends to ``report``."""
+    a capped coordinate descent appends to ``report``.  ``trace`` (a list) receives one record per view update
+    (oracle.sparse.update_record, what solve_penalised records and, for SCCA_IPLS, the std)."""
     m = len(dims)
     deltas = []
-    for _ in range(max_iter):
+    for it in range(max_iter):
         w_prev = [wi.copy() for wi in w]
         for i in range(m):
             raw, tn = cross(w, i)
+            rec = update_record(trace, it, i, raw, tn)
             if tn > 1e-12:
                 raw = raw / tn
             Gii = gram_ii(i)
-            wi = solve_penalised(Gii, raw / n, n, params[i][0], params[i][1], w[i], report=report)
+            wi = solve_penalised(Gii, raw / n, n, params[i][0], params[i][1], w[i], rcond=rcond, report=report, rec=rec)
             if kind == "ipls":
                 sd = np.sqrt(max(float(wi @ Gii @ wi) / n - float(colmean(i) @ wi) ** 2, 0.0))
+                if rec is not None:
+                    rec["sd"] = float(sd)
                 if sd > 1e-12:
                     wi = wi / sd
             w[i] = wi
@@ -103,11 +117,13 @@ def _loop(kind, dims, w, params, n, max_iter, tol, cross, gram_ii, colmean, repo
 
 
 def cov_elastic_fit(G, dims, n, kind, latent_dimensions=1, params=None, colmeans=None, init=None, max_iter=500,
-                    tol=1e-6, random_state=None, return_info=False):
+                    tol=1e-6, random_state=None, return_info=False, rcond=RCOND, trace=None):
     """ElasticCCA / SCCA_IPLS on the block Gram matrix G ((n - 1) C, centred or not following ``center``), the form
     csrc/als.cu iterates.  ``colmeans`` (D,): column means of the views, zeros (the default) when they are centred;
     deflated with the views.  Returns (weights per view (d_i x k), sweeps per dimension); as in ccab_als_fit, the sweep
-    count of a dimension in which a coordinate descent stopped at CD_SWEEPS above the KKT bound is negated."""
+    count of a dimension in which a coordinate descent stopped at CD_SWEEPS above the KKT bound is negated.  ``rcond``:
+    the relative eigenvalue cut of the lam = 0 solves (the ``mu`` of ops.als_fit); ``trace`` (a list) receives one
+    record per dimension (oracle.sparse.dimension_record)."""
     G = np.array(G, dtype=np.float64)
     dims = [int(p) for p in dims]
     m, k, D = len(dims), int(latent_dimensions), G.shape[0]
@@ -127,12 +143,15 @@ def cov_elastic_fit(G, dims, n, kind, latent_dimensions=1, params=None, colmeans
     for d in range(k):
         w = [v.copy() for v in init[d]]
         report = []
+        updates = None if trace is None else []
         deltas = _loop(kind, dims, w, params, n, max_iter, tol, cross, lambda i: G[sl[i], sl[i]], lambda i: mu[sl[i]],
-                       report)
+                       report, rcond, updates)
         iters.append(-len(deltas) if report else len(deltas))
         info.append(deltas)
         for i in range(m):
             W[i][:, d] = w[i]
+        if trace is not None:
+            trace.append(dimension_record(G, sl, w, updates, deltas))
         if d + 1 < k:
             E, F = np.zeros((D, m)), np.zeros((D, m))
             for i in range(m):

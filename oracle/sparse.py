@@ -44,24 +44,40 @@ def _soft(x, t):
     return np.sign(x) * np.maximum(np.abs(x) - t, 0.0)
 
 
-def _unit(x):
+def _unit(x, rec=None):
     nrm = np.linalg.norm(x)
+    if rec is not None:
+        rec["norm"] = float(nrm)
     return x / nrm if nrm > 1e-12 else x
 
 
-def _als_post(kind, raw, param):
-    """Per-view update from X_i^T t / ||t|| (the _update_weight of each Gauss-Seidel model)."""
+def tau_gap(x, t):
+    """min ||x_r| - t|: how far the soft-threshold support decision |x_r| > t is from flipping."""
+    return float(np.abs(np.abs(x) - t).min())
+
+
+def _als_post(kind, raw, param, rec=None):
+    """Per-view update from X_i^T t / ||t|| (the _update_weight of each Gauss-Seidel model).  ``rec`` (a dict) receives
+    the quantities its decisions turn on."""
     if kind == "parkhomenko":
-        return _unit(_soft(raw, param))
+        if rec is not None:
+            rec["tau_gap"] = tau_gap(raw, param)
+        return _unit(_soft(raw, param), rec)
     if kind == "span":
         if param < raw.size:
-            thr = np.sort(np.abs(raw))[-param]
+            srt = np.sort(np.abs(raw))
+            thr = srt[-param]
+            if rec is not None:
+                rec.update(thr=float(thr), gap=float(thr - srt[-param - 1]))
             raw = np.where(np.abs(raw) >= thr, raw, 0.0)
-        return _unit(raw)
+        return _unit(raw, rec)
     if kind == "pmd":
         bound = param
-        if np.abs(raw).sum() <= bound:
-            return _unit(raw)
+        l1 = np.abs(raw).sum()
+        if rec is not None:
+            rec.update(l1=float(l1), bound=float(bound))
+        if l1 <= bound:
+            return _unit(raw, rec)
         lo, hi = 0.0, float(np.abs(raw).max())
         for _ in range(50):
             mid = (lo + hi) / 2.0
@@ -69,15 +85,27 @@ def _als_post(kind, raw, param):
                 lo = mid
             else:
                 hi = mid
-        return _unit(_soft(raw, (lo + hi) / 2.0))
-    return _unit(raw)
+        if rec is not None:
+            rec.update(thr=(lo + hi) / 2.0, tau_gap=tau_gap(raw, (lo + hi) / 2.0))
+        return _unit(_soft(raw, (lo + hi) / 2.0), rec)
+    return _unit(raw, rec)
 
 
-def _als_loop(kind, dims, w, params, mu, n, max_iter, tol, cross, gram_ii):
+def update_record(trace, it, i, raw, tn):
+    """The record of one view update appended to ``trace`` (None without a trace): the raw target X_i^T t and ||t||."""
+    if trace is None:
+        return None
+    rec = {"sweep": it, "view": i, "raw": np.array(raw, dtype=np.float64), "tn": float(tn)}
+    trace.append(rec)
+    return rec
+
+
+def _als_loop(kind, dims, w, params, mu, n, max_iter, tol, cross, gram_ii, trace=None):
     """The iteration of one latent dimension, shared by the data-space and the Gram-space restatements.
 
     ``cross(w, i)`` -> (X_i^T t, ||t||) with t = sum_{j != i} X_j w_j;  ``gram_ii(i)`` -> X_i^T X_i.
-    Returns (sweeps, deltas)."""
+    Returns (sweeps, deltas).  ``trace`` (a list) receives one record per view update (update_record, plus what
+    the post-processing decides on)."""
     m = len(dims)
     deltas = []
     if kind == "admm":
@@ -89,6 +117,7 @@ def _als_loop(kind, dims, w, params, mu, n, max_iter, tol, cross, gram_ii):
             raws = [cross(w, i) for i in range(m)]
             for i in range(m):
                 raw, tn = raws[i]
+                rec = update_record(trace, it, i, raw, tn)
                 if tn > 1e-12:
                     raw = raw / tn
                 Gii = gram_ii(i)
@@ -96,6 +125,8 @@ def _als_loop(kind, dims, w, params, mu, n, max_iter, tol, cross, gram_ii):
                 w[i] = w[i] - g / (np.linalg.norm(Gii) / n + mu)
                 z[i] = _soft(w[i] + eta[i], params[i] / mu)
                 zn = np.linalg.norm(z[i])
+                if rec is not None:
+                    rec.update(zn=float(zn), tau_gap=tau_gap(w[i] + eta[i], params[i] / mu))
                 if zn > 1.0:
                     z[i] = z[i] / zn
                 eta[i] = eta[i] + w[i] - z[i]
@@ -104,9 +135,10 @@ def _als_loop(kind, dims, w, params, mu, n, max_iter, tol, cross, gram_ii):
         else:
             for i in range(m):
                 raw, tn = cross(w, i)
+                rec = update_record(trace, it, i, raw, tn)
                 if tn > 1e-12:
                     raw = raw / tn
-                w[i] = _als_post(kind, raw, params[i] * np.sqrt(dims[i]) if kind == "pmd" else params[i])
+                w[i] = _als_post(kind, raw, params[i] * np.sqrt(dims[i]) if kind == "pmd" else params[i], rec)
         delta = max(np.linalg.norm(w[i] - w_prev[i]) for i in range(m))
         deltas.append(delta)
         if delta < tol:
@@ -115,7 +147,7 @@ def _als_loop(kind, dims, w, params, mu, n, max_iter, tol, cross, gram_ii):
 
 
 def cov_als_fit(G, dims, n, kind, latent_dimensions=1, params=None, mu=1.0, init=None, max_iter=500, tol=1e-6,
-                random_state=None, return_info=False):
+                random_state=None, return_info=False, trace=None):
     """The sparse / ALS models on the block Gram matrix G = [X_1..X_m]^T [X_1..X_m] ((n - 1) C of the covariance the
     package computes, for either value of ``center``): the form csrc/als.cu iterates.
 
@@ -123,7 +155,7 @@ def cov_als_fit(G, dims, n, kind, latent_dimensions=1, params=None, mu=1.0, init
       deflation G <- Q^T G Q,  Q_i = I - w_i a_i^T / s_i
 
     Returns (weights per view (d_i x k), sweeps per dimension) and, with ``return_info``, the per-sweep convergence
-    deltas of every dimension."""
+    deltas of every dimension.  ``trace`` (a list) receives one record per dimension (dimension_record)."""
     G = np.array(G, dtype=np.float64)
     dims = [int(p) for p in dims]
     m, k = len(dims), int(latent_dimensions)
@@ -140,11 +172,15 @@ def cov_als_fit(G, dims, n, kind, latent_dimensions=1, params=None, mu=1.0, init
 
     for d in range(k):
         w = [v.copy() for v in init[d]]
-        sweeps, deltas = _als_loop(kind, dims, w, params, mu, n, max_iter, tol, cross, lambda i: G[sl[i], sl[i]])
+        updates = None if trace is None else []
+        sweeps, deltas = _als_loop(kind, dims, w, params, mu, n, max_iter, tol, cross, lambda i: G[sl[i], sl[i]],
+                                   updates)
         iters.append(sweeps)
         info.append(deltas)
         for i in range(m):
             W[i][:, d] = w[i]
+        if trace is not None:
+            trace.append(dimension_record(G, sl, w, updates, deltas))
         if d + 1 < k:
             D = G.shape[0]
             E, F = np.zeros((D, m)), np.zeros((D, m))
@@ -160,6 +196,13 @@ def cov_als_fit(G, dims, n, kind, latent_dimensions=1, params=None, mu=1.0, init
     if return_info:
         return W, iters, info
     return W, iters
+
+
+def dimension_record(G, sl, w, updates, deltas):
+    """The trace record of one latent dimension: max |G| of its (deflated) Gram matrix, its view updates, its
+    convergence deltas and the deflation scalars s_i = w_i^T G_ii w_i of its final weights."""
+    return {"gmax": float(np.abs(G).max()), "updates": updates, "deltas": list(deltas),
+            "s": [float(w[i] @ G[sl[i], sl[i]] @ w[i]) for i in range(len(sl))]}
 
 
 def ref_als_fit(views, kind, latent_dimensions=1, params=None, mu=1.0, max_iter=500, tol=1e-6, random_state=None,
