@@ -313,12 +313,18 @@ class BaseModel(BaseEstimator, ABC):
             n_local += state["n"]
         self._partial = {"mom": mom, "n": n_local, "dims": dims, "dtype": in_dtype}
         if solve:
-            if type(self)._requires_two_views and len(dims) != 2:
-                raise ValueError(f"rCCA requires exactly 2 views, got {len(dims)}. Use MCCA for more than 2 views.")
-            self._fit_moments(mom.clone(), n_local, dims, in_dtype)
+            self._fit_from_moments(mom.clone(), n_local, dims, in_dtype)
         return self
 
     _requires_two_views: ClassVar[bool] = False
+
+    def _fit_from_moments(self, mom, n_local, dims, in_dtype):
+        """Parameter validation, the view-count check and the solve from a moment buffer (consumed): the end of
+        ``partial_fit``, and how ``model_selection.GridSearchCV`` fits each candidate from a split's train moments."""
+        self._validate_params()
+        if type(self)._requires_two_views and len(dims) != 2:
+            raise ValueError(f"rCCA requires exactly 2 views, got {len(dims)}. Use MCCA for more than 2 views.")
+        return self._fit_moments(mom, n_local, dims, in_dtype)
 
     def __getstate__(self):
         """Estimators stay picklable like the reference's (SURVEY.md §5): fitted state is numpy; an open

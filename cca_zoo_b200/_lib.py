@@ -98,6 +98,9 @@ SIGNATURES = {
     "ccab_ccar3_admm_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "ccab_ccar3_admm": (C.c_int, [C.c_int, C.c_int, _vp, C.c_int64, _vp, C.c_int64, C.c_double, C.c_double, C.c_double,
                                   C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_size_t, _vp]),
+    "ccab_cv_scores_workspace_bytes": (C.c_size_t, [C.c_int, _i64p, C.c_int, C.c_int]),
+    "ccab_cv_scores": (C.c_int, [C.c_int, _i64p, _vp, C.c_int64, C.c_double, _vp, C.c_int64, C.c_int, C.c_int, _vp, _vp,
+                                 _vp, _vp, C.c_size_t, _vp]),
     "ccab_scale": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int64,
                              _vp]),
     "ccab_center_columns": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp]),

@@ -11,6 +11,7 @@
 #include "als.cuh"
 #include "ccaloss.cuh"
 #include "ccar3.cuh"
+#include "cv.cuh"
 #include "cholinv.cuh"
 #include "common.cuh"
 #include "gfa.cuh"
@@ -776,6 +777,39 @@ int ccab_ccar3_admm(int p, int q, const double* M, int64_t ldm, const double* B0
   if (rc) return rc;
   return ccar3_admm(p, q, M, ldm, B0, ldb, kappa, rho, tol, max_iter, Z, ldz, U, ldu, info, workspace,
                     workspace_bytes, static_cast<cudaStream_t>(stream));
+  CCAB_CATCH
+}
+
+size_t ccab_cv_scores_workspace_bytes(int n_views, const int64_t* dims, int G, int k_max) {
+  if (n_views < 2 || n_views > kMaxViews || !dims || G < 1 || k_max < 1) return 0;
+  for (int v = 0; v < n_views; ++v)
+    if (dims[v] < 1) return 0;
+  return cv_scores_workspace_bytes(n_views, dims, (int64_t)G * k_max);
+}
+
+int ccab_cv_scores(int n_views, const int64_t* dims, const double* C, int64_t ldc, double n, const double* W,
+                   int64_t ldw, int G, int k_max, const int* k_of, double* corr, double* score, void* workspace,
+                   size_t workspace_bytes, void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(n_views >= 2 && n_views <= kMaxViews, "cv_scores needs 2 to %d views, got %d", kMaxViews,
+                 n_views);
+  CCAB_CHECK_ARG(dims && C && W && k_of && corr && score && workspace, "null pointer argument");
+  int64_t D = 0;
+  for (int v = 0; v < n_views; ++v) {
+    CCAB_CHECK_ARG(dims[v] >= 1, "bad view width %lld", (long long)dims[v]);
+    D += dims[v];
+  }
+  CCAB_CHECK_ARG(D <= (1 << 20), "total width %lld is too large", (long long)D);
+  CCAB_CHECK_ARG(G >= 1 && k_max >= 1 && (int64_t)G * k_max <= (1 << 24), "bad candidate shape G = %d, k_max = %d", G,
+                 k_max);
+  CCAB_CHECK_ARG(ldc >= D && ldw >= (int64_t)G * k_max, "leading dimension too small");
+  CCAB_CHECK_ARG(n >= 2.0, "at least 2 held-out samples are needed, got n = %g", n);
+  CCAB_CHECK_ARG(workspace_bytes >= cv_scores_workspace_bytes(n_views, dims, (int64_t)G * k_max),
+                 "workspace too small: %zu bytes", workspace_bytes);
+  int rc = require_device();
+  if (rc) return rc;
+  return cv_scores(n_views, dims, C, ldc, n, W, ldw, G, k_max, k_of, corr, score, workspace,
+                   static_cast<cudaStream_t>(stream));
   CCAB_CATCH
 }
 

@@ -1079,3 +1079,39 @@ def ccar3_admm(M, B0, kappa: float, rho: float, tol: float, max_iter: int):
                                  _stream(M))
     _lib.check(rc, "ccab_ccar3_admm")
     return Z, U, info
+
+
+def cv_scores(C, dims, n, W, k_of):
+    """Held-out scores of G fitted candidates (ccab_cv_scores): ``C`` is the float64 D x D covariance of ``n`` held-out
+    rows (CUDA), ``W`` the D x G k_max float64 weights (CUDA, row-major, candidate b's dimension j in column
+    b k_max + j, zero past its width), ``k_of`` the G widths (host ints, 1 <= k_of[b] <= k_max).  Returns (corr
+    (G x k_max), score (G)) float64 CUDA tensors: the average off-diagonal pairwise correlation per dimension and its
+    mean over each candidate's dimensions."""
+    lib = _lib.load()
+    _require_cuda(C, "C")
+    _require_cuda(W, "W")
+    dims = [int(p) for p in dims]
+    D, G = sum(dims), len(k_of)
+    if not 2 <= len(dims) <= _lib.MAX_VIEWS:
+        raise ValueError(f"cv_scores takes 2 to {_lib.MAX_VIEWS} views, got {len(dims)}")
+    if G < 1 or W.dim() != 2 or W.shape[1] % G != 0 or W.shape[1] == 0:
+        raise ValueError(f"W must have G k_max columns for G = {G} candidates, got shape {tuple(W.shape)}")
+    k_max = int(W.shape[1]) // G
+    if any(not 1 <= int(k) <= k_max for k in k_of):
+        raise ValueError(f"every candidate width must lie in 1..{k_max}, got {list(k_of)}")
+    for t, name, cols in ((C, "C", D), (W, "W", G * k_max)):
+        if t.dtype != torch.float64 or t.dim() != 2 or tuple(t.shape) != ((D, D) if name == "C" else (D, cols)):
+            raise ValueError(f"{name} must be a float64 {D} x {cols} matrix, got {t.dtype} {tuple(t.shape)}")
+    if not n >= 2:
+        raise ValueError(f"at least 2 held-out samples are needed, got n = {n}")
+    C, W = _row_major(C, False), _row_major(W, False)
+    d = _lib.i64_array(dims)
+    ws = _ws(lib.ccab_cv_scores_workspace_bytes(len(dims), d, G, k_max), C.device)
+    kk = torch.tensor([int(k) for k in k_of], dtype=torch.int32).to(C.device, non_blocking=True)
+    corr = torch.empty((G, k_max), dtype=torch.float64, device=C.device)
+    score = torch.empty(G, dtype=torch.float64, device=C.device)
+    with torch.cuda.device(C.device):
+        rc = lib.ccab_cv_scores(len(dims), d, _ptr(C), C.stride(0), float(n), _ptr(W), W.stride(0), G, k_max, _ptr(kk),
+                                _ptr(corr), _ptr(score), _ptr(ws), ws.numel(), _stream(C))
+    _lib.check(rc, "ccab_cv_scores")
+    return corr, score

@@ -439,6 +439,21 @@ int ccab_ccar3_admm(int p, int q, const double* M, int64_t ldm, const double* B0
                     double rho, double tol, int max_iter, double* Z, int64_t ldz, double* U, int64_t ldu,
                     double* info, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- held-out scores of a batch of fitted candidates (the cross-validation scoring of GridSearchCV) --------------
+ * C (device, D x D float64, ldc) is the covariance of n held-out rows, D = sum(dims), 2 <= n_views <= CCAB_MAX_VIEWS.
+ * W (device, D x G k_max float64, row-major, ldw) packs G candidates: column b k_max + j holds dimension j of candidate
+ * b (the views' weight blocks stacked by rows), zero past k_of[b] (device int32[G], 1 <= k_of[b] <= k_max).
+ * corr (device, G x k_max) receives the average off-diagonal pairwise correlation of the projected rows per dimension
+ * (zero past k_of[b]), score (device, G) its mean over the first k_of[b] dimensions: per pair
+ * S_il = w_i^T C_il w_l / (den_i den_l) with den_i = sqrt(S_ii (n - 1)), or 1 when that is <= 1e-12, over sqrt(n - 1).
+ * The products C[:, block l] W[block l, :] run on the fp64 tensor pipe; every sum has a fixed order, so repeated calls
+ * are bit-identical.  workspace_bytes is 0 for arguments the entry point refuses.
+ * Replaces one clone / fit / score cycle's score(), cca_zoo/_base.py:153-194, per candidate and split. */
+size_t ccab_cv_scores_workspace_bytes(int n_views, const int64_t* dims, int G, int k_max);
+int ccab_cv_scores(int n_views, const int64_t* dims, const double* C, int64_t ldc, double n, const double* W,
+                   int64_t ldw, int G, int k_max, const int* k_of, double* corr, double* score, void* workspace,
+                   size_t workspace_bytes, void* stream);
+
 /* ---- the deep-CCA objective behind the ABI (any widths) ---------------------------------------------------------
  * ccab_ccaloss_fwd: loss[0] = -|| S11^-1/2 S12 S22^-1/2 ||_F^2 with S_ii = cov(z_i) + eps I, from the moment pass over
  * [z1 z2] (precision as in ccab_moments), a batched Cholesky + inverse and 7 GEMMs; `saved`
