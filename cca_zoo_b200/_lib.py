@@ -86,6 +86,8 @@ SIGNATURES = {
     "ccab_tcca_moment_workspace_bytes": (C.c_size_t, [C.c_int, _i64p, C.c_int64, C.c_int]),
     "ccab_tcca_moment": (C.c_int, [C.c_int, _i64p, C.c_int64, C.POINTER(_vp), _i64p, C.c_double, C.c_int, _vp, _vp,
                                    C.c_size_t, _vp]),
+    "ccab_tcca_moment_adjoint": (C.c_int, [C.c_int, _i64p, C.c_int64, _vp, C.POINTER(_vp), _i64p, C.c_double, _vp,
+                                           C.POINTER(_vp), _i64p, _vp]),
     "ccab_tcca_state_size": (C.c_int64, [C.c_int, _i64p, C.c_int]),
     "ccab_tcca_fit_workspace_bytes": (C.c_size_t, [C.c_int, _i64p, C.c_int]),
     "ccab_tcca_fit": (C.c_int, [C.c_int, _i64p, C.c_int, _vp, C.POINTER(_vp), _vp, _vp, C.c_int, C.c_int, _vp, _vp,

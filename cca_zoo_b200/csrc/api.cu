@@ -707,6 +707,28 @@ int ccab_tcca_moment(int n_views, const int64_t* dims, int64_t n, const double* 
   CCAB_CATCH
 }
 
+int ccab_tcca_moment_adjoint(int n_views, const int64_t* dims, int64_t n, const double* M, const double* const* H,
+                             const int64_t* ldh, double scale, const double* scale_dev, double* const* Y,
+                             const int64_t* ldy, void* stream) {
+  CCAB_TRY
+  int rc = tcca_check_dims(n_views, dims);
+  if (rc) return rc;
+  CCAB_CHECK_ARG(n >= 1, "krprod_adjoint needs at least one sample, got n = %lld", (long long)n);
+  CCAB_CHECK_ARG(H && ldh && Y && ldy && M, "null pointer argument");
+  for (int i = 0; i < n_views; ++i) {
+    CCAB_CHECK_ARG(dims[i] <= (int64_t)65535 * 64, "view %d has width %lld; the adjoint supports at most %d", i,
+                   (long long)dims[i], 65535 * 64);
+    CCAB_CHECK_ARG(H[i] && ldh[i] >= dims[i], "H[%d]: null pointer or leading dimension %lld < width %lld", i,
+                   (long long)ldh[i], (long long)dims[i]);
+    CCAB_CHECK_ARG(Y[i] && ldy[i] >= dims[i], "Y[%d]: null pointer or leading dimension %lld < width %lld", i,
+                   (long long)ldy[i], (long long)dims[i]);
+  }
+  rc = require_device();
+  if (rc) return rc;
+  return tcca_moment_adjoint(n_views, dims, n, M, H, ldh, scale, scale_dev, Y, ldy, static_cast<cudaStream_t>(stream));
+  CCAB_CATCH
+}
+
 int64_t ccab_tcca_state_size(int n_views, const int64_t* dims, int k) {
   if (tcca_check_dims(n_views, dims)) return -1;
   if (k < 1 || k > kTccaMaxK) {

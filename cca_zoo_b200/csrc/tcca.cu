@@ -219,6 +219,175 @@ int tcca_moment(int n_views, const int64_t* dims, int64_t n, const double* const
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Khatri-Rao adjoint
+// ---------------------------------------------------------------------------------------------------------------
+struct KrAdjArgs {
+  const double* H[kTccaMaxViews];
+  int64_t ldh[kTccaMaxViews];
+  double* Y[kTccaMaxViews];
+  int64_t ldy[kTccaMaxViews];
+  int p[kTccaMaxViews];
+  int stride[kTccaMaxViews];    // C-order strides of M
+  int nv;
+  int64_t n;
+  double scale;
+  const double* dscale;         // optional device factor
+  const double* M;
+};
+
+// Y_i = f * KR_{j != i}(H_j) M_(i)^T for the mode i = blockIdx.z: a 64 x 64 tile (samples x mode-i index) of an
+// (n x P_i) x (P_i x k_i) product, with the tiling of krprod_moment_kernel.  The reduction runs over the positions
+// of the other modes (C order, the last of them fastest) in steps of 16; each thread owns one position q of the step
+// and tracks its multi-index as mixed-radix digits, advanced by the digits of 16 with one conditional subtraction per
+// digit.  From it the thread generates the KR entries of 4 samples (the A slice) and reads M at 4 mode-i indices
+// through the mode-i stride (the B slice): no permuted copy of M.  One CTA owns the whole reduction of its tile, so
+// the summation order is fixed.
+__global__ void __launch_bounds__(256) krprod_adjoint_kernel(const KrAdjArgs a) {
+  constexpr int KC = 16, LDS = 64 + 4;
+  __shared__ double As[2][KC][LDS];   // [position][sample]
+  __shared__ double Bs[2][KC][LDS];   // [position][mode-i index]
+  const int mode = blockIdx.z, ki = a.p[mode];
+  const int64_t m0 = (int64_t)blockIdx.x * 64;
+  const int n0 = blockIdx.y * 64;
+  if (n0 >= ki) return;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wm = (warp & 1) * 32, wn = (warp >> 1) * 16;
+  const int gq = lane >> 2, tq = lane & 3;
+  const int q = tid & 15, g = tid >> 4;
+  const int64_t si = a.stride[mode];
+  int P = 1;
+#pragma unroll
+  for (int v = 0; v < kTccaMaxViews; ++v)
+    if (v < a.nv && v != mode) P *= a.p[v];
+  // digits of q and of the step 16 (both mod P) over the other modes
+  int dig[kTccaMaxViews], inc[kTccaMaxViews];
+  {
+    int r0 = q % P, r1 = KC % P;
+#pragma unroll
+    for (int v = kTccaMaxViews - 1; v >= 0; --v) {
+      dig[v] = inc[v] = 0;
+      if (v < a.nv && v != mode) {
+        dig[v] = r0 % a.p[v];
+        r0 /= a.p[v];
+        inc[v] = r1 % a.p[v];
+        r1 /= a.p[v];
+      }
+    }
+  }
+
+  double ra[4], rb[4];
+  auto load_regs = [&](int k0) {
+    const bool in = k0 + q < P;
+    int64_t off = 0;
+#pragma unroll
+    for (int v = 0; v < kTccaMaxViews; ++v)
+      if (v < a.nv && v != mode) off += (int64_t)dig[v] * a.stride[v];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int64_t s = m0 + g + 16 * r;
+      double x = 0.0;
+      if (in && s < a.n) {
+        x = 1.0;
+#pragma unroll
+        for (int v = 0; v < kTccaMaxViews; ++v)
+          if (v < a.nv && v != mode) x *= a.H[v][s * a.ldh[v] + dig[v]];
+      }
+      ra[r] = x;
+      const int c = n0 + 4 * g + r;
+      rb[r] = (in && c < ki) ? a.M[off + c * si] : 0.0;
+    }
+    int carry = 0;
+#pragma unroll
+    for (int v = kTccaMaxViews - 1; v >= 0; --v) {
+      if (v < a.nv && v != mode) {
+        const int d = dig[v] + inc[v] + carry;
+        carry = d >= a.p[v];
+        dig[v] = carry ? d - a.p[v] : d;
+      }
+    }
+  };
+  auto store_regs = [&](int buf) {
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      As[buf][q][g + 16 * r] = ra[r];
+      Bs[buf][q][4 * g + r] = rb[r];
+    }
+  };
+
+  double acc[4][2][2];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
+
+  load_regs(0);
+  store_regs(0);
+  __syncthreads();
+  int buf = 0;
+  for (int k0 = 0; k0 < P; k0 += KC) {
+    const bool more = k0 + KC < P;
+    if (more) load_regs(k0 + KC);
+#pragma unroll
+    for (int kk = 0; kk < KC; kk += 4) {
+      double fa[4], fb[2];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) fa[i] = As[buf][kk + tq][wm + 8 * i + gq];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) fb[j] = Bs[buf][kk + tq][wn + 8 * j + gq];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) tcca_dmma_884(acc[i][j][0], acc[i][j][1], fa[i], fb[j]);
+    }
+    if (more) {
+      store_regs(buf ^ 1);
+      __syncthreads();
+      buf ^= 1;
+    }
+  }
+  const double f = a.dscale ? a.scale * *a.dscale : a.scale;
+  double* Y = a.Y[mode];
+  const int64_t ldy = a.ldy[mode];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int64_t r = m0 + wm + 8 * i + gq;
+        const int c = n0 + wn + 8 * j + 2 * tq + e;
+        if (r < a.n && c < ki) Y[r * ldy + c] = f * acc[i][j][e];
+      }
+}
+
+int tcca_moment_adjoint(int n_views, const int64_t* dims, int64_t n, const double* M, const double* const* H,
+                        const int64_t* ldh, double scale, const double* dscale, double* const* Y, const int64_t* ldy,
+                        cudaStream_t stream) {
+  KrAdjArgs a = {};
+  a.nv = n_views;
+  int64_t P = 1, kmax = 1;
+  for (int i = n_views - 1; i >= 0; --i) {
+    a.H[i] = H[i];
+    a.ldh[i] = ldh[i];
+    a.Y[i] = Y[i];
+    a.ldy[i] = ldy[i];
+    a.p[i] = (int)dims[i];
+    a.stride[i] = (int)P;
+    P *= dims[i];
+    kmax = std::max<int64_t>(kmax, dims[i]);
+  }
+  a.n = n;
+  a.scale = scale;
+  a.dscale = dscale;
+  a.M = M;
+  dim3 grid((unsigned)ceil_div(n, 64), (unsigned)ceil_div(kmax, 64), (unsigned)n_views);
+  krprod_adjoint_kernel<<<grid, 256, 0, stream>>>(a);
+  count_launches(1);
+  CCAB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // CP-ALS
 // ---------------------------------------------------------------------------------------------------------------
 struct AlsArgs {

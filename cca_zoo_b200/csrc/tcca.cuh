@@ -22,6 +22,10 @@ size_t tcca_moment_workspace_bytes(int n_views, const int64_t* dims, int64_t n, 
 int tcca_moment(int n_views, const int64_t* dims, int64_t n, const double* const* Z, const int64_t* ldz, double scale,
                 int nsplit, double* M, void* ws, size_t ws_bytes, cudaStream_t stream);
 
+int tcca_moment_adjoint(int n_views, const int64_t* dims, int64_t n, const double* M, const double* const* H,
+                        const int64_t* ldh, double scale, const double* dscale, double* const* Y, const int64_t* ldy,
+                        cudaStream_t stream);
+
 size_t tcca_state_doubles(int n_views, const int64_t* dims, int k);
 size_t tcca_fit_workspace_bytes(int n_views, const int64_t* dims, int k);
 int tcca_fit(int n_views, const int64_t* dims, int k, const double* M, const double* const* evecs, const double* lam0,

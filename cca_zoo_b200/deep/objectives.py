@@ -384,3 +384,186 @@ class GCCALoss(nn.Module):
     def forward(self, representations: list[torch.Tensor]) -> torch.Tensor:
         prec = _resolve_precision(self.precision, [_row_major(z) for z in representations])
         return _GCCALossFn.apply(float(self.eps), prec, *representations)
+
+
+def _tcca_divided_differences(lam, eps):
+    """F_ab = (f(l_a) - f(l_b)) / (l_a - l_b), F_aa = f'(l_a) for f(l) = max(l, eps)^-1/2 (f' = 0 where the clamp is
+    active); where both eigenvalues are unclamped the closed form -1 / (s_a s_b (s_a + s_b)), s = sqrt(l), which has
+    no cancellation and is the finite limit at a repeated eigenvalue."""
+    s = lam.clamp_min(eps).sqrt()
+    f = 1.0 / s
+    la, lb = lam[:, None], lam[None, :]
+    d = la - lb
+    mixed = torch.where(d != 0, (f[:, None] - f[None, :]) / torch.where(d != 0, d, torch.ones_like(d)),
+                        torch.zeros_like(d))
+    both = (la > eps) & (lb > eps)
+    return torch.where(both, -1.0 / (s[:, None] * s[None, :] * (s[:, None] + s[None, :])), mixed)
+
+
+def _tcca_eigen_whiten(C, z64, off, dims, eps):
+    """clamp(eigh(S_i), min=eps) whitening, S_i = C_ii + eps I, literally: H_i = Zc_i W_i, W_i = V f(Lam) V^T.
+    Returns the H_i and, per view, what the backward needs: (Zc_i, W_i, V^T, F)."""
+    H, parts = [], []
+    for i, d in enumerate(dims):
+        lam, Vt = ops.syevj(C[off[i]:off[i + 1], off[i]:off[i + 1]].clone())
+        Wt, _, _ = ops.whiten_rows(lam, Vt, 0.0, floor_add=eps, rank_tol=-1.0, lam_floor=0.0)
+        W = ops.gemm(Vt, Wt, transa=True)
+        Zc = ops.center_columns_(z64[i].clone())
+        H.append(ops.gemm(Zc, W))
+        parts.append((Zc, W, Vt, _tcca_divided_differences(lam + eps, eps)))
+    return H, parts
+
+
+class _TCCALossFn(torch.autograd.Function):
+    """-||M||_F, M = (1/n) sum_s H_1[s] x ... x H_m[s], in float64 for every input dtype (see TCCALoss)."""
+
+    @staticmethod
+    def forward(ctx, eps, precision, status, sync, *zs):
+        dt = zs[0].dtype
+        n, m = int(zs[0].shape[0]), len(zs)
+        zd = [_row_major(z) for z in zs]
+        dims = [int(z.shape[1]) for z in zd]
+        off = [0]
+        for d in dims:
+            off.append(off[-1] + d)
+        mom = ops.moments(zd, precision=_resolve_precision(precision, zd))
+        C, _ = ops.covariance(mom, dims, n, center=True, dtype=torch.float64)
+        z64 = [z if z.dtype == torch.float64 else z.to(torch.float64) for z in zd]
+        eigen = n - 1 < max(dims)                      # rank deficient by shape: the clamp is active for certain
+        if eigen and not bool(torch.isfinite(C).all()):       # the eigen route reads back anyway
+            raise ValueError("TCCALoss: a representation contained NaN or infinity.")
+        if not eigen:
+            Linv, flags = [], []
+            if len(set(dims)) == 1:                    # one batched factorisation for all views
+                S = torch.stack([C[off[i]:off[i + 1], off[i]:off[i + 1]] for i in range(m)])
+                S.diagonal(dim1=1, dim2=2).add_(eps)
+                L, info = ops.potrf_inv_(S, pivot_tol=0.25 * eps)
+                Linv, flags = [L[i] for i in range(m)], [info]
+            else:
+                for i in range(m):
+                    S = C[off[i]:off[i + 1], off[i]:off[i + 1]].clone()    # C stays intact for the eigen route
+                    S.diagonal().add_(eps)
+                    L, info = ops.potrf_inv_(S, pivot_tol=0.25 * eps)
+                    Linv.append(L)
+                    flags.append(info)
+            flags.append((~torch.isfinite(C).all()).to(torch.int32).reshape(1))
+            flags = torch.cat(flags)
+            # H_i = Zc_i R_i with R_i = L_i^-T: centring commutes with the right factor
+            H = [ops.center_columns_(ops.gemm(z, L, transb=True)) for z, L in zip(z64, Linv)]
+            if sync:
+                f = flags.tolist()                     # verify='sync': one read-back per step
+                if f[-1]:
+                    raise ValueError("TCCALoss: a representation contained NaN or infinity.")
+                eigen = any(f[:-1])
+            else:
+                status.push(flags)
+        if eigen:
+            if dt != torch.float64:    # the clamp at eps is decided on the eigenvalues: float64 moments for those
+                C, _ = ops.covariance(ops.moments(z64), dims, n, center=True, dtype=torch.float64)
+            H, parts = _tcca_eigen_whiten(C, z64, off, dims, eps)
+        M = ops.tcca_moment(H)
+        norm = ops.frobenius_norm(M)
+        ctx.n, ctx.m, ctx.dt, ctx.eigen = n, m, dt, eigen
+        saved = [M, norm, *H]
+        if eigen:
+            for p in parts:
+                saved += list(p)
+        else:
+            saved += Linv
+        ctx.save_for_backward(*saved)
+        return (-norm).reshape(()).to(dt).clone()
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        n, m = ctx.n, ctx.m
+        t = ctx.saved_tensors
+        M, norm, H = t[0], t[1], t[2:2 + m]
+        rest = t[2 + m:]
+        go = grad_out.to(torch.float64).reshape(1)
+        # Gamma_i = dL/dH_i = -Y_i / (n ||M||) * grad_out; 0 at ||M|| = 0 (torch's subgradient of the norm)
+        coef = torch.where(norm > 0, -go / (n * norm), torch.zeros_like(norm))
+        gam = ops.tcca_moment_adjoint(M, list(H), scale_dev=coef)
+        grads = []
+        for i in range(m):
+            g = gam[i]
+            if ctx.eigen:
+                Zc, W, Vt, F = rest[4 * i:4 * i + 4]
+                B = ops.gemm(Zc, g, transa=True)
+                B = 0.5 * (B + B.T)
+                X = ops.gemm(Vt, F * ops.gemm(ops.gemm(Vt, B), Vt, transb=True), transa=True)
+                X = ops.gemm(X, Vt)
+                out = ops.gemm(g, W)
+                ops.gemm(Zc, X, alpha=2.0 / (n - 1), beta=1.0, out=out)
+                ops.center_columns_(out)
+            else:
+                # (Gamma_i - H_i (H_i^T Gamma_i) / (n - 1)) R_i^T, centred; R_i^T = L_i^-1
+                T = ops.gemm(H[i], g, transa=True)
+                ops.gemm(H[i], T, alpha=-1.0 / (n - 1), beta=1.0, out=g)
+                ops.center_columns_(g)
+                out = ops.gemm(g, rest[i])
+            grads.append(out.to(ctx.dt))
+        return (None, None, None, None, *grads)
+
+
+class TCCALoss(nn.Module):
+    r"""Deep tensor-CCA loss for 2 to 8 views (cca_zoo/deep/objectives.py:223-289): :math:`-\|M\|_F` with
+    :math:`M = \frac1n \sum_s H_1[s] \otimes \cdots \otimes H_m[s]` the cross-moment tensor of the whitened
+    representations :math:`H_i = \tilde Z_i\,\mathrm{clamp}(S_i)^{-1/2}`, :math:`S_i = \mathrm{cov}(z_i) + \epsilon I`.
+    Views may have different widths; the product of the widths is at most 2^25.  Plugs into ``DTCCA``, which sets
+    its objective in its constructor: assign ``model.objective = TCCALoss(eps=model.eps)`` afterwards.
+
+    The reference materialises the n x k_1 x ... x k_m outer-product array and keeps it for autograd.  Here M is
+    contracted on the fp64 tensor pipe without that array (``ccab_tcca_moment``), and the backward is analytic: one
+    launch of the Khatri-Rao adjoint (``ccab_tcca_moment_adjoint``) gives every dL/dH_i, then a few k_i x k_i
+    products per view.  ||M||_F does not change under an orthogonal change of basis in any mode, so the whitening is
+    a Cholesky factor of S_i, which equals the reference whenever its eigenvalue clamp is inactive; batches that are
+    rank deficient by shape (n - 1 < k_i) take the eigen route, the reference's ``clamp(eigh(S_i), min=eps)``
+    literally.  All of it runs in float64, also for float32 representations (the moment pass then follows
+    ``precision``); the loss and the gradients come back in the input dtype.  Where some S_i has a repeated
+    eigenvalue (a constant representation: S_i = eps I) the reference's eigh backward returns NaN; the gradient here
+    is the finite limit.  ||M||_F = 0 gives a zero gradient.
+
+    Args:
+        eps: ridge added to the within-view covariances and eigenvalue floor (default 1e-5).
+        precision: arithmetic of the moment pass for float32 inputs, as in ``CCALoss``.
+        verify: ``"lazy"`` (default) reads nothing back: the Cholesky status and a NaN flag are inspected at the next
+            call or by ``check()``.  ``"sync"`` reads them back in every call, raises ``ValueError`` on NaN or
+            infinity and takes the eigen route for a batch whose S_i is not numerically positive definite.
+    """
+
+    def __init__(self, eps: float = 1e-5, precision: str = "auto", verify: str = "lazy") -> None:
+        super().__init__()
+        if verify not in ("lazy", "sync"):
+            raise ValueError("verify must be 'lazy' or 'sync'")
+        self.eps = eps
+        self.precision = precision
+        self.verify = verify
+        self._status = _LazyStatus("TCCALoss")
+
+    def check(self) -> None:
+        """Wait for the status of every evaluation issued so far and raise if one of them was unreliable."""
+        self._status.check()
+
+    def forward(self, representations: list[torch.Tensor]) -> torch.Tensor:
+        zs = list(representations)
+        if not 2 <= len(zs) <= ops.TCCA_MAX_VIEWS:
+            raise ValueError(f"TCCALoss takes 2 to {ops.TCCA_MAX_VIEWS} representations, got {len(zs)}.")
+        _require_cuda("TCCALoss", *zs)
+        dt = zs[0].dtype
+        if dt not in (torch.float32, torch.float64) or any(z.dtype != dt for z in zs):
+            raise ValueError("representations must share a float32/float64 dtype")
+        if any(z.dim() != 2 for z in zs) or any(z.shape[0] != zs[0].shape[0] for z in zs):
+            raise ValueError("representations must be 2-D with the same number of rows")
+        n = int(zs[0].shape[0])
+        if n < 2:
+            raise ValueError(f"TCCALoss needs at least 2 samples for a covariance, got n = {n}.")
+        entries = 1
+        for z in zs:
+            if z.shape[1] < 1:
+                raise ValueError("every representation needs at least one column")
+            entries *= int(z.shape[1])
+        if entries > ops.TCCA_MAX_ENTRIES:
+            raise ValueError(f"the cross-moment tensor of widths {[int(z.shape[1]) for z in zs]} has {entries} entries; "
+                             f"TCCALoss supports at most 2^25 = {ops.TCCA_MAX_ENTRIES} (the product of the widths).")
+        self._status.poll()
+        return _TCCALossFn.apply(float(self.eps), self.precision, self._status, self.verify == "sync", *zs)

@@ -873,6 +873,43 @@ def tcca_moment(Z, nsplit: int = 0):
     return M
 
 
+def tcca_moment_adjoint(M, H, scale: float = 1.0, scale_dev=None):
+    """[Y_i] with Y_i = f * KR_{j != i}(H_j) M_(i)^T (n x p_i float64, CUDA) for every mode i, in one launch
+    (ccab_tcca_moment_adjoint): the adjoint of ``tcca_moment`` in each of its modes.  ``M`` holds the tensor in C order
+    (prod p_i entries, e.g. the output of ``tcca_moment``), ``H`` the float64 (n, p_i) CUDA views; f = ``scale``
+    times the one-element float64 CUDA tensor ``scale_dev`` when given (it is never read back)."""
+    lib = _lib.load()
+    _require_cuda(M, "M")
+    for i, h in enumerate(H):
+        _require_cuda(h, f"H[{i}]")
+    H = [_row_major(h, False) for h in H]
+    if M.dtype != torch.float64 or any(h.dtype != torch.float64 for h in H):
+        raise ValueError("tcca_moment_adjoint takes a float64 tensor and float64 views")
+    n = int(H[0].shape[0])
+    if any(int(h.shape[0]) != n for h in H):
+        raise ValueError("tcca_moment_adjoint: the views differ in their number of rows")
+    dims = [int(h.shape[1]) for h in H]
+    P = 1
+    for p in dims:
+        P *= p
+    if M.numel() != P:
+        raise ValueError(f"M must have {P} entries (the product of the view widths {dims}), got {M.numel()}")
+    if scale_dev is not None:
+        _require_cuda(scale_dev, "scale_dev")
+        if scale_dev.dtype != torch.float64 or scale_dev.numel() != 1:
+            raise ValueError("scale_dev must be a one-element float64 tensor")
+    M = M.contiguous()
+    Y = [torch.empty((n, p), dtype=torch.float64, device=M.device) for p in dims]
+    m = len(dims)
+    hp = (C.c_void_p * m)(*[h.data_ptr() for h in H])
+    yp = (C.c_void_p * m)(*[y.data_ptr() for y in Y])
+    with torch.cuda.device(M.device):
+        rc = lib.ccab_tcca_moment_adjoint(m, _lib.i64_array(dims), n, _ptr(M), hp, _lib.i64_array([h.stride(0) for h in H]),
+                                          float(scale), _ptr(scale_dev), yp, _lib.i64_array(dims), _stream(M))
+    _lib.check(rc, "ccab_tcca_moment_adjoint")
+    return Y
+
+
 def tcca_layout(dims, k: int) -> dict:
     """Offsets (doubles) of the state block of ccab_tcca_fit: ``rec``, ``F`` (one per mode), ``G`` and ``total``."""
     at = TCCA_HEADER + TCCA_MAX_ITER

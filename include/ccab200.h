@@ -359,6 +359,22 @@ size_t ccab_tcca_moment_workspace_bytes(int n_views, const int64_t* dims, int64_
 int ccab_tcca_moment(int n_views, const int64_t* dims, int64_t n, const double* const* Z, const int64_t* ldz,
                      double scale, int nsplit, double* M, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ccab_tcca_moment_adjoint: the adjoint of the contraction of ccab_tcca_moment in every mode, in one launch:
+ *   Y[i] = f * KR_{j != i}(H_j) M_(i)^T,   Y[i][s, a] = f * sum_{idx: idx_i = a} M[idx] prod_{j != i} H_j[s, idx_j],
+ * f = scale * (*scale_dev) (scale alone when scale_dev is NULL; scale_dev is a device double, never read back).
+ * M is the tensor in C order (prod p_i float64 entries, as ccab_tcca_moment writes it), read through the mode-i
+ * strides: no permuted copy.  H[i] are float64 n x p_i row-major device matrices (leading dimension ldh[i] >= p_i),
+ * Y[i] float64 n x p_i row-major outputs (ldy[i] >= p_i).  Each (n x P_i) x (P_i x p_i) product, P_i = prod_{j != i}
+ * p_j, runs on the fp64 tensor pipe (DMMA) with the Khatri-Rao operand generated in shared memory from the H_j rows,
+ * never stored.  Every output tile sums its whole reduction in one fixed order, with no splits and no atomics:
+ * repeated calls are bit-identical, and no workspace is needed.
+ * Needs 2 <= n_views <= 8, 1 <= p_i <= 65535 * 64, prod p_i <= 2^25, n >= 1.
+ * With M = ccab_tcca_moment(H) at scale 1/n and f = 1/n, Y[i] is the gradient of ||M||_F^2 / 2 with respect to
+ * H_i: the backward of the deep tensor-CCA objective (TCCALoss). */
+int ccab_tcca_moment_adjoint(int n_views, const int64_t* dims, int64_t n, const double* M, const double* const* H,
+                             const int64_t* ldh, double scale, const double* scale_dev, double* const* Y,
+                             const int64_t* ldy, void* stream);
+
 /* ccab_tcca_fit: up to n_iter iterations of tensorly's parafac ALS (unnormalised, exact solve per mode, stop when
  * |rec_prev - rec| < 1e-8 from the second iteration on, at most 100 iterations in all) on the tensor M (float64,
  * prod p_i entries in C order), asynchronous: a fixed launch sequence in which every kernel returns at once once the
