@@ -41,6 +41,7 @@ SIGNATURES = {
     "ccab_shift_rows": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int, C.c_int64, _vp, _vp, C.c_int64, _vp]),
     "ccab_moments_unshift": (C.c_int, [C.c_int, C.c_int, _i64p, _vp, C.POINTER(_vp), C.c_double, _vp]),
     "ccab_covariance": (C.c_int, [C.c_int, C.c_int, _i64p, _vp, C.c_double, C.c_int, _vp, C.c_int64, _vp, _vp]),
+    "ccab_covariance_ndev": (C.c_int, [C.c_int, C.c_int, _i64p, _vp, _vp, C.c_int, _vp, C.c_int64, _vp, _vp]),
     "ccab_syevj_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "ccab_syevj": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, C.c_int64, C.c_double, _vp, _vp, C.c_int64,
                              C.POINTER(C.c_int), C.POINTER(C.c_float), _vp, C.c_size_t, _vp]),
@@ -69,6 +70,11 @@ SIGNATURES = {
                                    C.c_double, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
     "ccab_ccaloss_bwd": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int, C.c_int, _vp, _vp, _vp,
                                    C.c_int64, _vp, C.c_int64, _vp]),
+    "ccab_ccaloss_fwd_moments_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "ccab_ccaloss_fwd_moments": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, _vp, C.c_double, _vp, _vp, _vp, _vp,
+                                           C.c_size_t, _vp]),
+    "ccab_ccaloss_bwd_global": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int, C.c_int, _vp,
+                                          _vp, _vp, C.c_int64, _vp, C.c_int64, _vp]),
     "ccab_mcca_fit_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, _i64p, C.c_int, C.c_int]),
     "ccab_mcca_fit_result_layout": (C.c_int, [C.c_int, C.c_int, _i64p, C.c_int, C.c_int, _i64p]),
     "ccab_mcca_fit": (C.c_int, [C.c_int, C.c_int, _i64p, _vp, _vp, C.c_double, C.c_int, C.POINTER(C.c_double),
@@ -106,6 +112,7 @@ SIGNATURES = {
     "ccab_scale": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int64,
                              _vp]),
     "ccab_center_columns": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp]),
+    "ccab_row_sub_scale": (C.c_int, [C.c_int, C.c_int64, C.c_int, _vp, C.c_int64, _vp, _vp, _vp]),
     "ccab_frobenius_norm": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, C.c_int64, _vp, _vp]),
     "ccab_profile_moments": (C.c_int, [C.c_int]),
     "ccab_profile_moments_last_ms": (C.c_double, []),

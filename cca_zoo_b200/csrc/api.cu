@@ -228,6 +228,25 @@ int ccab_covariance(int out_dtype, int n_views, const int64_t* dims, const doubl
   CCAB_CATCH
 }
 
+int ccab_covariance_ndev(int out_dtype, int n_views, const int64_t* dims, const double* moments, const double* n_dev,
+                         int center, void* C, int64_t ldc, void* mean, void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(out_dtype == CCAB_F32 || out_dtype == CCAB_F64, "bad dtype %d", out_dtype);
+  CCAB_CHECK_ARG(dims && moments && n_dev && C, "null pointer argument");
+  ColumnLayout L;
+  int rc = make_layout(n_views, dims, &L);
+  if (rc) return rc;
+  rc = require_device();
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (out_dtype == CCAB_F32)
+    return covariance_from_moments_ndev<float>(L, moments, n_dev, center, static_cast<float*>(C), ldc,
+                                               static_cast<float*>(mean), s);
+  return covariance_from_moments_ndev<double>(L, moments, n_dev, center, static_cast<double*>(C), ldc,
+                                              static_cast<double*>(mean), s);
+  CCAB_CATCH
+}
+
 size_t ccab_syevj_workspace_bytes(int dtype, int n, int batch) {
   if (n < 1 || batch < 1) return 0;
   return dtype == CCAB_F32 ? jacobi_workspace_bytes<float>(n, n, batch) : jacobi_workspace_bytes<double>(n, n, batch);
@@ -552,6 +571,56 @@ int ccab_ccaloss_bwd(int dtype, const void* z1, int64_t ld1, const void* z2, int
   return ccaloss_backward<double>(d1, d2, static_cast<const double*>(z1), ld1, static_cast<const double*>(z2), ld2, n,
                                   static_cast<const double*>(saved), static_cast<const double*>(grad_out),
                                   static_cast<double*>(g1), ldg1, static_cast<double*>(g2), ldg2, s);
+  CCAB_CATCH
+}
+
+size_t ccab_ccaloss_fwd_moments_workspace_bytes(int dtype, int d1, int d2) {
+  int64_t dims[2] = {d1, d2};
+  ColumnLayout L;
+  if (make_layout(2, dims, &L)) return 0;
+  return dtype == CCAB_F32 ? ccaloss_fwd_moments_workspace_bytes<float>(L) : ccaloss_fwd_moments_workspace_bytes<double>(L);
+}
+
+int ccab_ccaloss_fwd_moments(int dtype, int d1, int d2, const double* moments, const double* n_dev, double eps,
+                             void* loss, void* saved, int* flags_dev, void* workspace, size_t workspace_bytes,
+                             void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
+  CCAB_CHECK_ARG(moments && n_dev && loss && saved && flags_dev && workspace, "null pointer argument");
+  int64_t dims[2] = {d1, d2};
+  ColumnLayout L;
+  int rc = make_layout(2, dims, &L);
+  if (rc) return rc;
+  rc = require_device();
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (dtype == CCAB_F32)
+    return ccaloss_forward_moments<float>(L, moments, n_dev, eps, static_cast<float*>(loss), static_cast<float*>(saved),
+                                          flags_dev, workspace, workspace_bytes, s);
+  return ccaloss_forward_moments<double>(L, moments, n_dev, eps, static_cast<double*>(loss),
+                                         static_cast<double*>(saved), flags_dev, workspace, workspace_bytes, s);
+  CCAB_CATCH
+}
+
+int ccab_ccaloss_bwd_global(int dtype, const void* z1, int64_t ld1, const void* z2, int64_t ld2, int64_t n_local, int d1,
+                            int d2, const void* saved, const void* grad_out, void* g1, int64_t ldg1, void* g2,
+                            int64_t ldg2, void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
+  CCAB_CHECK_ARG(saved && (n_local == 0 || (z1 && z2 && g1 && g2)), "null pointer argument");
+  CCAB_CHECK_ARG(ld1 >= d1 && ld2 >= d2 && ldg1 >= d1 && ldg2 >= d2, "leading dimension too small");
+  int rc = require_device();
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (dtype == CCAB_F32)
+    return ccaloss_backward_global<float>(d1, d2, static_cast<const float*>(z1), ld1, static_cast<const float*>(z2),
+                                          ld2, n_local, static_cast<const float*>(saved),
+                                          static_cast<const float*>(grad_out), static_cast<float*>(g1), ldg1,
+                                          static_cast<float*>(g2), ldg2, s);
+  return ccaloss_backward_global<double>(d1, d2, static_cast<const double*>(z1), ld1, static_cast<const double*>(z2),
+                                         ld2, n_local, static_cast<const double*>(saved),
+                                         static_cast<const double*>(grad_out), static_cast<double*>(g1), ldg1,
+                                         static_cast<double*>(g2), ldg2, s);
   CCAB_CATCH
 }
 
@@ -912,6 +981,22 @@ int ccab_center_columns(int dtype, int m, int n, void* A, int64_t lda, void* str
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (dtype == CCAB_F32) return center_columns<float>(m, n, static_cast<float*>(A), lda, s);
   return center_columns<double>(m, n, static_cast<double*>(A), lda, s);
+  CCAB_CATCH
+}
+
+int ccab_row_sub_scale(int dtype, int64_t m, int n, void* A, int64_t lda, const void* r, const void* s_dev,
+                       void* stream) {
+  CCAB_TRY
+  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
+  CCAB_CHECK_ARG(A != nullptr || m == 0 || n == 0, "null pointer argument");
+  int rc = require_device();
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (dtype == CCAB_F32)
+    return row_sub_scale<float>(m, n, static_cast<float*>(A), lda, static_cast<const float*>(r),
+                                static_cast<const float*>(s_dev), s);
+  return row_sub_scale<double>(m, n, static_cast<double*>(A), lda, static_cast<const double*>(r),
+                               static_cast<const double*>(s_dev), s);
   CCAB_CATCH
 }
 

@@ -290,9 +290,10 @@ __device__ void chol_inverse_pair(T* A1, int d1, T* A2, int d2, T* X1, T* X2, T*
 }
 
 template <typename T>
-__global__ void __launch_bounds__(1024) ccaloss_small_fwd_kernel(const double* __restrict__ mom, int Dp, double n, int d1,
-                                                                 int d2, T eps, T* __restrict__ loss,
-                                                                 T* __restrict__ saved, int* __restrict__ flags) {
+__global__ void __launch_bounds__(1024) ccaloss_small_fwd_kernel(const double* __restrict__ mom, int Dp, double n_host,
+                                                                 const double* __restrict__ n_dev, int d1, int d2,
+                                                                 T eps, T* __restrict__ loss, T* __restrict__ saved,
+                                                                 int* __restrict__ flags) {
   extern __shared__ __align__(16) unsigned char ccl_smem[];
   T* I1 = reinterpret_cast<T*>(ccl_smem);   // S11 -> S11^-1
   T* I2 = I1 + kLD * kLP;                    // S22 -> S22^-1
@@ -315,6 +316,7 @@ __global__ void __launch_bounds__(1024) ccaloss_small_fwd_kernel(const double* _
     I1[i * kLP + j] = I2[i * kLP + j] = (i == j) ? T(1) : T(0);
   }
   __syncthreads();
+  const double n = n_dev ? n_dev[0] : n_host;    // global batch: the all-reduced count, read on the device
   const double inv = 1.0 / (n - 1.0), inv_n = 1.0 / n;
   int notfinite = 0;
   for (int e = threadIdx.x; e < d1 * d1; e += blockDim.x) {
@@ -341,6 +343,7 @@ __global__ void __launch_bounds__(1024) ccaloss_small_fwd_kernel(const double* _
   T* G22 = Pout + (size_t)d1 * d2;
   T* mean = G22 + (size_t)d2 * d2;
   for (int i = threadIdx.x; i < d1 + d2; i += blockDim.x) mean[i] = (T)(s[i < d1 ? i : o2 + i - d1] * inv_n);
+  if (n_dev && threadIdx.x == 0) mean[d1 + d2] = (T)n;   // global batch: N rides behind the means for the backward
   __syncthreads();
   chol_inverse_pair(I1, d1, I2, d2, Tm, Tm2, Pm, rowk, T(0.25) * eps, notpd);
   smem_matmul4<T, 0, 0>(I1, S12, Tm, d1, d2, d1);      // Tm  = A1 S12          (Q)
@@ -378,7 +381,8 @@ __global__ void __launch_bounds__(256) ccaloss_small_bwd_kernel(int d1, int d2, 
                                                                 const T* __restrict__ z2, int64_t ld2, int64_t n,
                                                                 const T* __restrict__ saved,
                                                                 const T* __restrict__ grad_out, T* __restrict__ g1,
-                                                                int64_t ldg1, T* __restrict__ g2, int64_t ldg2) {
+                                                                int64_t ldg1, T* __restrict__ g2, int64_t ldg2,
+                                                                bool global) {
   extern __shared__ __align__(16) unsigned char ccb_smem[];
   T* G11 = reinterpret_cast<T*>(ccb_smem);   // [64][65] each
   T* Ps = G11 + kLD * kLP;
@@ -424,7 +428,9 @@ __global__ void __launch_bounds__(256) ccaloss_small_bwd_kernel(int d1, int d2, 
   }
   __syncthreads();
   const int r = tid >> 2, q = tid & 3;
-  const T scale = (T)(2.0 / (double)(n - 1)) * (grad_out ? grad_out[0] : T(1));
+  // global batch: n counts this shard's rows only; the scale takes the all-reduced N saved behind the means
+  const double nm1 = global ? (double)smean[d1 + d2] - 1.0 : (double)(n - 1);
+  const T scale = (T)(2.0 / nm1) * (grad_out ? grad_out[0] : T(1));
   T a1[16], a2[16];
 #pragma unroll
   for (int j = 0; j < 16; ++j) a1[j] = a2[j] = T(0);
@@ -458,7 +464,7 @@ __global__ void __launch_bounds__(256) ccaloss_small_bwd_kernel(int d1, int d2, 
 
 template <typename T>
 int ccaloss_small_forward(const double* moments, int Dp, double n, int d1, int d2, double eps, T* loss, T* saved,
-                          int* flags, cudaStream_t stream) {
+                          int* flags, cudaStream_t stream, const double* n_dev) {
   CCAB_CHECK_ARG(d1 >= 1 && d2 >= 1 && d1 <= kLD && d2 <= kLD && Dp == 256, "ccaloss_small_forward: widths 1..64");
   const size_t smem = sizeof(T) * (6 * kLD * kLP + 4 * kLD + 40);
   static bool attr_done[64] = {};
@@ -468,7 +474,7 @@ int ccaloss_small_forward(const double* moments, int Dp, double n, int d1, int d
     CCAB_CUDA(cudaFuncSetAttribute(ccaloss_small_fwd_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (dev >= 0 && dev < 64) attr_done[dev] = true;
   }
-  ccaloss_small_fwd_kernel<T><<<1, 1024, smem, stream>>>(moments, Dp, n, d1, d2, (T)eps, loss, saved, flags);
+  ccaloss_small_fwd_kernel<T><<<1, 1024, smem, stream>>>(moments, Dp, n, n_dev, d1, d2, (T)eps, loss, saved, flags);
   count_launches(1);
   CCAB_CUDA(cudaGetLastError());
   return 0;
@@ -477,8 +483,10 @@ int ccaloss_small_forward(const double* moments, int Dp, double n, int d1, int d
 template <typename T>
 int ccaloss_small_backward(int d1, int d2, const T* z1, int64_t ld1, const T* z2, int64_t ld2, int64_t n,
                            const T* saved, const T* grad_out, T* g1, int64_t ldg1, T* g2, int64_t ldg2,
-                           cudaStream_t stream) {
-  CCAB_CHECK_ARG(d1 >= 1 && d2 >= 1 && d1 <= kLD && d2 <= kLD && n >= 2, "ccaloss_small_backward: widths 1..64");
+                           cudaStream_t stream, bool global) {
+  CCAB_CHECK_ARG(d1 >= 1 && d2 >= 1 && d1 <= kLD && d2 <= kLD && n >= (global ? 0 : 2),
+                 "ccaloss_small_backward: widths 1..64");
+  if (n == 0) return 0;                            // a rank without rows in a global batch
   const size_t smem = sizeof(T) * (5 * kLD * kLP + 4 * kLD);
   static bool attr_done[64] = {};
   int dev = 0;
@@ -488,21 +496,21 @@ int ccaloss_small_backward(int d1, int d2, const T* z1, int64_t ld1, const T* z2
     if (dev >= 0 && dev < 64) attr_done[dev] = true;
   }
   ccaloss_small_bwd_kernel<T><<<(unsigned)ceil_div(n, 64), 256, smem, stream>>>(d1, d2, z1, ld1, z2, ld2, n, saved,
-                                                                                grad_out, g1, ldg1, g2, ldg2);
+                                                                                grad_out, g1, ldg1, g2, ldg2, global);
   count_launches(1);
   CCAB_CUDA(cudaGetLastError());
   return 0;
 }
 
 template int ccaloss_small_forward<float>(const double*, int, double, int, int, double, float*, float*, int*,
-                                          cudaStream_t);
+                                          cudaStream_t, const double*);
 template int ccaloss_small_forward<double>(const double*, int, double, int, int, double, double*, double*, int*,
-                                           cudaStream_t);
+                                           cudaStream_t, const double*);
 template int ccaloss_small_backward<float>(int, int, const float*, int64_t, const float*, int64_t, int64_t, const float*,
-                                           const float*, float*, int64_t, float*, int64_t, cudaStream_t);
+                                           const float*, float*, int64_t, float*, int64_t, cudaStream_t, bool);
 template int ccaloss_small_backward<double>(int, int, const double*, int64_t, const double*, int64_t, int64_t,
                                             const double*, const double*, double*, int64_t, double*, int64_t,
-                                            cudaStream_t);
+                                            cudaStream_t, bool);
 
 template int ccaloss_small<float>(const float*, int64_t, int, int, double, float*, float*, float*, float*, float*,
                                   cudaStream_t);

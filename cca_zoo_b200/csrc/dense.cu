@@ -476,6 +476,32 @@ int center_columns(int m, int n, T* A, int64_t lda, cudaStream_t stream) {
 template int center_columns<float>(int, int, float*, int64_t, cudaStream_t);
 template int center_columns<double>(int, int, double*, int64_t, cudaStream_t);
 
+// one thread per element of a 32-column strip, grid-stride over the rows
+template <typename T>
+__global__ void row_sub_scale_kernel(int64_t m, int n, T* __restrict__ A, int64_t lda, const T* __restrict__ r,
+                                     const T* __restrict__ s) {
+  const int j = blockIdx.x * 32 + (threadIdx.x & 31);
+  if (j >= n) return;
+  const T rj = r[j], sc = s[0];
+  for (int64_t i = (int64_t)blockIdx.y * (blockDim.x >> 5) + (threadIdx.x >> 5); i < m;
+       i += (int64_t)gridDim.y * (blockDim.x >> 5))
+    A[i * lda + j] = (A[i * lda + j] - rj) * sc;
+}
+
+template <typename T>
+int row_sub_scale(int64_t m, int n, T* A, int64_t lda, const T* r, const T* s, cudaStream_t stream) {
+  CCAB_CHECK_ARG(m >= 0 && n >= 0 && lda >= n, "row_sub_scale: bad shape");
+  CCAB_CHECK_ARG(r && s, "row_sub_scale: r and s are required");
+  if (m == 0 || n == 0) return 0;
+  const unsigned gy = (unsigned)std::min<int64_t>(ceil_div(m, 8), 1024);
+  row_sub_scale_kernel<T><<<dim3((unsigned)ceil_div(n, 32), gy), 256, 0, stream>>>(m, n, A, lda, r, s);
+  count_launches(1);
+  CCAB_CUDA(cudaGetLastError());
+  return 0;
+}
+template int row_sub_scale<float>(int64_t, int, float*, int64_t, const float*, const float*, cudaStream_t);
+template int row_sub_scale<double>(int64_t, int, double*, int64_t, const double*, const double*, cudaStream_t);
+
 // Two passes in one CTA.  Pass 1 finds max |a| and the exponent e that puts max |a| 2^-e in [0.5, 1); pass 2 sums
 // (a 2^-e)^2 in a fixed order and the norm is 2^e sqrt(sum).  The scaling is exact and moves every square by the even
 // power 2^-2e, so at ordinary scales the result is sqrt(sum a^2) bit for bit, while the squares can neither overflow

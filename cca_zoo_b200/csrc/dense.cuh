@@ -52,6 +52,10 @@ int scale_rows_cols(int m, int n, const T* A, int64_t lda, const T* r, int r_pow
 template <typename T>
 int center_columns(int m, int n, T* A, int64_t lda, cudaStream_t stream);
 
+// A[i, :] = (A[i, :] - r) * s[0]   (m x n row-major, in place; r: device T[n], s: device T[1])
+template <typename T>
+int row_sub_scale(int64_t m, int n, T* A, int64_t lda, const T* r, const T* s, cudaStream_t stream);
+
 // out[0] = ||A||_F (m x n, row-major)
 template <typename T>
 int frobenius_norm(int m, int n, const T* A, int64_t lda, T* out, cudaStream_t stream);

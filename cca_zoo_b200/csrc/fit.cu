@@ -893,13 +893,14 @@ struct LossPlan {
   int d1, d2, D, Dp;
   int64_t ldC, ldR, strideR;
   bool batched;
-  size_t oMom, oMomWs, oC, oR, oLinv, oA, oQ, oQ2, oPws, oSmall, total;
+  size_t oMom, oMomWs, oC, oR, oLinv, oA, oQ, oQ2, oPws, oSmall, oMean, total;
   size_t mom_ws_bytes, pws_bytes;
   size_t sG11, sP, sG22, s_total;   // element offsets inside `saved`
 };
 
+// from_moments: the stage after a given (all-reduced) moment buffer -- no moment sections, a double[D] for the means
 template <typename T>
-LossPlan make_loss_plan(const ColumnLayout& L, int64_t n, int precision) {
+LossPlan make_loss_plan(const ColumnLayout& L, int64_t n, int precision, bool from_moments = false) {
   LossPlan P;
   P.d1 = L.dims[0]; P.d2 = L.dims[1]; P.D = L.D; P.Dp = L.Dp;
   P.ldC = r4(P.D);
@@ -909,10 +910,17 @@ LossPlan make_loss_plan(const ColumnLayout& L, int64_t n, int precision) {
   P.batched = P.d1 == P.d2;
   size_t o = 0;
   auto take = [&](size_t bytes) { size_t at = o; o += al256(bytes); return at; };
-  P.oMom = take(sizeof(double) * ((size_t)P.Dp * P.Dp + P.Dp));
-  P.mom_ws_bytes = std::max(moments_workspace_bytes(std::is_same<T, float>::value ? 0 : 1, precision, L, n),
-                            moments_workspace_bytes(std::is_same<T, float>::value ? 0 : 1, 2, L, n)) + 512;
-  P.oMomWs = take(P.mom_ws_bytes);
+  if (from_moments) {
+    P.oMom = P.oMomWs = 0;
+    P.mom_ws_bytes = 0;
+    P.oMean = take(sizeof(double) * (size_t)P.D);
+  } else {
+    P.oMom = take(sizeof(double) * ((size_t)P.Dp * P.Dp + P.Dp));
+    P.mom_ws_bytes = std::max(moments_workspace_bytes(std::is_same<T, float>::value ? 0 : 1, precision, L, n),
+                              moments_workspace_bytes(std::is_same<T, float>::value ? 0 : 1, 2, L, n)) + 512;
+    P.oMomWs = take(P.mom_ws_bytes);
+    P.oMean = 0;
+  }
   P.oC = take(sizeof(T) * (size_t)P.D * P.ldC);
   P.oR = take(sizeof(T) * 2 * (size_t)P.strideR);
   P.oLinv = take(sizeof(T) * 2 * (size_t)P.strideR);
@@ -937,15 +945,23 @@ size_t ccaloss_workspace_bytes(const ColumnLayout& L, int64_t n, int precision) 
   return make_loss_plan<T>(L, n, precision).total;
 }
 
+namespace {
+
+// saved[0 .. D) = (T) mean, saved[D] = (T) N: the global means and count behind G11 | P | G22 (wide global forward)
 template <typename T>
-int ccaloss_forward(const ColumnLayout& L, int precision, const void* z1, int64_t ld1, const void* z2, int64_t ld2,
-                    int64_t n, double eps, T* loss, T* saved, int* flags_out, void* ws, size_t ws_bytes, cudaStream_t s) {
-  CCAB_CHECK_ARG(L.n_views == 2 && n >= 2, "ccaloss_forward: two views and at least 2 samples");
-  LossPlan P = make_loss_plan<T>(L, n, precision);
-  CCAB_CHECK_ARG(ws_bytes >= P.total, "ccaloss workspace too small: %zu < %zu", ws_bytes, P.total);
-  uint8_t* w = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
+__global__ void saved_tail_kernel(const double* __restrict__ mean, int D, const double* __restrict__ n_dev,
+                                  T* __restrict__ tail) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= D; i += gridDim.x * blockDim.x)
+    tail[i] = (T)(i < D ? mean[i] : n_dev[0]);
+}
+
+// Wide widths, everything after the moment pass: covariance + ridge blocks, batched Cholesky + inverse, 7 GEMMs, loss.
+// n_dev == NULL: n_host rows (the fused local forward).  n_dev != NULL: an all-reduced buffer whose count is read on the
+// device; the global means and N are appended to `saved` for ccaloss_backward_global.
+template <typename T>
+int loss_stage(const LossPlan& P, const ColumnLayout& L, uint8_t* w, const double* mom, const double* n_dev, double n_host,
+               double eps, T* loss, T* saved, int* flags_out, cudaStream_t s) {
   const int d1 = P.d1, d2 = P.d2, D = P.D;
-  double* mom = reinterpret_cast<double*>(w + P.oMom);
   T* C = reinterpret_cast<T*>(w + P.oC);
   T* R1 = reinterpret_cast<T*>(w + P.oR);
   T* R2 = R1 + P.strideR;
@@ -964,22 +980,8 @@ int ccaloss_forward(const ColumnLayout& L, int precision, const void* z1, int64_
   T* Pm = saved + P.sP;
   T* G22 = saved + P.sG22;
 
-  // ---- moments of [z1 z2] ----
-  const void* views[2] = {z1, z2};
-  const int64_t lds[2] = {ld1, ld2};
+  double* mean = n_dev ? reinterpret_cast<double*>(w + P.oMean) : nullptr;
   int rc;
-  if (std::max(d1, d2) <= 64) {
-    // narrow representations (config 3's k = 64): the moment pass (exact FMA, HBM / latency bound) and ONE single-CTA
-    // launch for everything else
-    rc = moments_simt<T>(L, views, lds, n, mom, w + P.oMomWs, P.mom_ws_bytes, s);
-    if (rc) return rc;
-    return ccaloss_small_forward<T>(mom, L.Dp, (double)n, d1, d2, eps, loss, saved, flags_out, s);
-  }
-  if (std::is_same<T, float>::value && precision != 2)
-    rc = moments_tf32(L, views, lds, n, precision, mom, w + P.oMomWs, P.mom_ws_bytes, s);
-  else
-    rc = moments_simt<T>(L, views, lds, n, mom, w + P.oMomWs, P.mom_ws_bytes, s);
-  if (rc) return rc;
   CCAB_CUDA(cudaMemsetAsync(sm, 0, 1024, s));
   {
     CovRidgeParams cp;
@@ -989,7 +991,7 @@ int ccaloss_forward(const ColumnLayout& L, int precision, const void* z1, int64_
     for (int v = 0; v <= 2; ++v) { cp.coff[v] = L.coff[v]; cp.poff[v] = L.poff[v]; }
     cp.R[0] = R1; cp.R[1] = R2; cp.ldr[0] = ldr1; cp.ldr[1] = ldr2;
     dim3 block(32, 8), grid((unsigned)ceil_div(D, 32), (unsigned)ceil_div(D, 8));
-    cov_ridge_kernel<T><<<grid, block, 0, s>>>(cp, mom, nullptr, (double)n, 1, C, P.ldC, nullptr, dmax, flags + 4);
+    cov_ridge_kernel<T><<<grid, block, 0, s>>>(cp, mom, n_dev, n_host, 1, C, P.ldC, mean, dmax, flags + 4);
     count_launches(1);
     CCAB_CUDA(cudaGetLastError());
   }
@@ -1052,10 +1054,63 @@ int ccaloss_forward(const ColumnLayout& L, int precision, const void* z1, int64_
     count_launches(2);
   }
   CCAB_CUDA(cudaGetLastError());
+  if (n_dev) {
+    saved_tail_kernel<T><<<1, 256, 0, s>>>(mean, D, n_dev, saved + P.s_total);
+    count_launches(1);
+    CCAB_CUDA(cudaGetLastError());
+  }
   // flags_out[0..1] = Cholesky status, [2] = non-finite moments
   CCAB_CUDA(cudaMemcpyAsync(flags_out, flags, 2 * sizeof(int), cudaMemcpyDeviceToDevice, s));
   CCAB_CUDA(cudaMemcpyAsync(flags_out + 2, flags + 4, sizeof(int), cudaMemcpyDeviceToDevice, s));
   return 0;
+}
+
+}  // namespace
+
+template <typename T>
+int ccaloss_forward(const ColumnLayout& L, int precision, const void* z1, int64_t ld1, const void* z2, int64_t ld2,
+                    int64_t n, double eps, T* loss, T* saved, int* flags_out, void* ws, size_t ws_bytes, cudaStream_t s) {
+  CCAB_CHECK_ARG(L.n_views == 2 && n >= 2, "ccaloss_forward: two views and at least 2 samples");
+  LossPlan P = make_loss_plan<T>(L, n, precision);
+  CCAB_CHECK_ARG(ws_bytes >= P.total, "ccaloss workspace too small: %zu < %zu", ws_bytes, P.total);
+  uint8_t* w = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
+  const int d1 = P.d1, d2 = P.d2;
+  double* mom = reinterpret_cast<double*>(w + P.oMom);
+
+  // ---- moments of [z1 z2] ----
+  const void* views[2] = {z1, z2};
+  const int64_t lds[2] = {ld1, ld2};
+  int rc;
+  if (std::max(d1, d2) <= 64) {
+    // narrow representations (config 3's k = 64): the moment pass (exact FMA, HBM / latency bound) and ONE single-CTA
+    // launch for everything else
+    rc = moments_simt<T>(L, views, lds, n, mom, w + P.oMomWs, P.mom_ws_bytes, s);
+    if (rc) return rc;
+    return ccaloss_small_forward<T>(mom, L.Dp, (double)n, d1, d2, eps, loss, saved, flags_out, s);
+  }
+  if (std::is_same<T, float>::value && precision != 2)
+    rc = moments_tf32(L, views, lds, n, precision, mom, w + P.oMomWs, P.mom_ws_bytes, s);
+  else
+    rc = moments_simt<T>(L, views, lds, n, mom, w + P.oMomWs, P.mom_ws_bytes, s);
+  if (rc) return rc;
+  return loss_stage<T>(P, L, w, mom, nullptr, (double)n, eps, loss, saved, flags_out, s);
+}
+
+template <typename T>
+size_t ccaloss_fwd_moments_workspace_bytes(const ColumnLayout& L) {
+  return make_loss_plan<T>(L, 0, 2, true).total;
+}
+
+template <typename T>
+int ccaloss_forward_moments(const ColumnLayout& L, const double* mom, const double* n_dev, double eps, T* loss,
+                            T* saved, int* flags_out, void* ws, size_t ws_bytes, cudaStream_t s) {
+  CCAB_CHECK_ARG(L.n_views == 2 && mom && n_dev, "ccaloss_forward_moments: two views, a moment buffer and n_dev");
+  LossPlan P = make_loss_plan<T>(L, 0, 2, true);
+  CCAB_CHECK_ARG(ws_bytes >= P.total, "ccaloss workspace too small: %zu < %zu", ws_bytes, P.total);
+  uint8_t* w = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
+  if (std::max(P.d1, P.d2) <= 64)
+    return ccaloss_small_forward<T>(mom, L.Dp, 0.0, P.d1, P.d2, eps, loss, saved, flags_out, s, n_dev);
+  return loss_stage<T>(P, L, w, mom, n_dev, 0.0, eps, loss, saved, flags_out, s);
 }
 
 template <typename T>
@@ -1114,6 +1169,106 @@ int ccaloss_backward(int d1, int d2, const T* z1, int64_t ld1, const T* z2, int6
   return 0;
 }
 
+namespace {
+
+// Epilogue of the global backward, for g_v = z_v G_vv - z_w P^(T) over this shard's rows (blockIdx.z = v): subtract the
+// column means of the whole batch's products, r_1 = mu_1^T G11 - mu_2^T P^T, r_2 = mu_2^T G22 - mu_1^T P (a small product
+// of the saved global means), and scale by 2/(N-1) grad_out with N saved behind the means.  Each block recomputes r for
+// its 32 columns (8 row groups over the contraction, added in group order: every block gets the same bits), then
+// rewrites its slab of rows.
+template <typename T>
+__global__ void __launch_bounds__(256) ccaloss_global_center_kernel(int64_t m, int d1, int d2, T* __restrict__ g1,
+                                                                    int64_t ldg1, T* __restrict__ g2, int64_t ldg2,
+                                                                    const T* __restrict__ saved,
+                                                                    const T* __restrict__ grad_out, int rows_per_block) {
+  __shared__ double part[8][33];
+  const int v = blockIdx.z;
+  const int d = v ? d2 : d1, dw = v ? d1 : d2;
+  const int lane = threadIdx.x & 31, rg = threadIdx.x >> 5;
+  const int j = blockIdx.x * 32 + lane;
+  if (blockIdx.x * 32 >= d) return;                  // uniform over the block
+  const T* G11 = saved;
+  const T* Pm = G11 + (size_t)d1 * d1;
+  const T* G22 = Pm + (size_t)d1 * d2;
+  const T* mu = G22 + (size_t)d2 * d2;               // mu_1 | mu_2 | N
+  const T* Gv = v ? G22 : G11;
+  const T* mv = v ? mu + d1 : mu;
+  const T* mw = v ? mu : mu + d1;
+  double acc = 0.0;
+  if (j < d) {
+    for (int k = rg; k < d; k += 8) acc += (double)mv[k] * (double)Gv[(size_t)k * d + j];
+    // v = 0: (mu_2^T P^T)_j = sum_k mu_2[k] P[j][k];  v = 1: (mu_1^T P)_j = sum_k mu_1[k] P[k][j]
+    for (int k = rg; k < dw; k += 8)
+      acc -= (double)mw[k] * (double)(v ? Pm[(size_t)k * d2 + j] : Pm[(size_t)j * d2 + k]);
+  }
+  part[rg][lane] = acc;
+  __syncthreads();
+  if (rg == 0) {
+    double t = 0.0;
+    for (int k = 0; k < 8; ++k) t += part[k][lane];
+    part[0][lane] = t;
+  }
+  __syncthreads();
+  if (j >= d) return;
+  const T r = (T)part[0][lane];
+  const T sc = (T)(2.0 / ((double)mu[d1 + d2] - 1.0)) * (grad_out ? grad_out[0] : T(1));
+  T* g = v ? g2 : g1;
+  const int64_t ldg = v ? ldg2 : ldg1;
+  const int64_t r0 = (int64_t)blockIdx.y * rows_per_block, r1 = min(m, r0 + (int64_t)rows_per_block);
+  for (int64_t i = r0 + rg; i < r1; i += 8) g[i * ldg + j] = (g[i * ldg + j] - r) * sc;
+}
+
+}  // namespace
+
+template <typename T>
+int ccaloss_backward_global(int d1, int d2, const T* z1, int64_t ld1, const T* z2, int64_t ld2, int64_t n,
+                            const T* saved, const T* grad_out, T* g1, int64_t ldg1, T* g2, int64_t ldg2,
+                            cudaStream_t s) {
+  CCAB_CHECK_ARG(n >= 0 && d1 >= 1 && d2 >= 1, "ccaloss_backward_global: bad shape");
+  if (n == 0) return 0;                              // a rank without rows: nothing to write
+  if (std::max(d1, d2) <= 64)
+    return ccaloss_small_backward<T>(d1, d2, z1, ld1, z2, ld2, n, saved, grad_out, g1, ldg1, g2, ldg2, s, true);
+  const T* G11 = saved;
+  const T* Pm = saved + (size_t)d1 * d1;
+  const T* G22 = Pm + (size_t)d1 * d2;
+  GemmArgs<T> g;   // g1 = z1 G11
+  g.m = (int)n; g.n = d1; g.k = d1; g.A = z1; g.lda = ld1; g.B = G11; g.ldb = d1; g.C = g1; g.ldc = ldg1;
+  int rc = xgemm<T>(g, s);
+  if (rc) return rc;
+  GemmArgs<T> h;   // g1 -= z2 P^T
+  h.transb = 1; h.m = (int)n; h.n = d1; h.k = d2; h.alpha = T(-1); h.beta = T(1);
+  h.A = z2; h.lda = ld2; h.B = Pm; h.ldb = d2; h.C = g1; h.ldc = ldg1;
+  rc = xgemm<T>(h, s);
+  if (rc) return rc;
+  GemmArgs<T> u;   // g2 = z2 G22
+  u.m = (int)n; u.n = d2; u.k = d2; u.A = z2; u.lda = ld2; u.B = G22; u.ldb = d2; u.C = g2; u.ldc = ldg2;
+  rc = xgemm<T>(u, s);
+  if (rc) return rc;
+  GemmArgs<T> v;   // g2 -= z1 P
+  v.m = (int)n; v.n = d2; v.k = d1; v.alpha = T(-1); v.beta = T(1);
+  v.A = z1; v.lda = ld1; v.B = Pm; v.ldb = d2; v.C = g2; v.ldc = ldg2;
+  rc = xgemm<T>(v, s);
+  if (rc) return rc;
+  const int row_blocks = (int)std::min<int64_t>(64, ceil_div(n, 64));
+  const int rows_per_block = (int)ceil_div(n, row_blocks);
+  dim3 grid((unsigned)ceil_div(std::max(d1, d2), 32), (unsigned)row_blocks, 2);
+  ccaloss_global_center_kernel<T><<<grid, 256, 0, s>>>(n, d1, d2, g1, ldg1, g2, ldg2, saved, grad_out, rows_per_block);
+  count_launches(1);
+  CCAB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+template size_t ccaloss_fwd_moments_workspace_bytes<float>(const ColumnLayout&);
+template size_t ccaloss_fwd_moments_workspace_bytes<double>(const ColumnLayout&);
+template int ccaloss_forward_moments<float>(const ColumnLayout&, const double*, const double*, double, float*, float*,
+                                            int*, void*, size_t, cudaStream_t);
+template int ccaloss_forward_moments<double>(const ColumnLayout&, const double*, const double*, double, double*,
+                                             double*, int*, void*, size_t, cudaStream_t);
+template int ccaloss_backward_global<float>(int, int, const float*, int64_t, const float*, int64_t, int64_t,
+                                            const float*, const float*, float*, int64_t, float*, int64_t, cudaStream_t);
+template int ccaloss_backward_global<double>(int, int, const double*, int64_t, const double*, int64_t, int64_t,
+                                             const double*, const double*, double*, int64_t, double*, int64_t,
+                                             cudaStream_t);
 template size_t ccaloss_workspace_bytes<float>(const ColumnLayout&, int64_t, int);
 template size_t ccaloss_workspace_bytes<double>(const ColumnLayout&, int64_t, int);
 template int ccaloss_forward<float>(const ColumnLayout&, int, const void*, int64_t, const void*, int64_t, int64_t, double,

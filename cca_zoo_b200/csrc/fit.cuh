@@ -50,4 +50,19 @@ template <typename T>
 int ccaloss_backward(int d1, int d2, const T* z1, int64_t ld1, const T* z2, int64_t ld2, int64_t n, const T* saved,
                      const T* grad_out, T* g1, int64_t ldg1, T* g2, int64_t ldg2, cudaStream_t stream);
 
+// ---- global batch (moments all-reduced over data-parallel ranks) ----
+// The stage of ccaloss_forward after the moment pass, from a given buffer whose sample count N is read at n_dev[0]
+// (device).  saved (T[d1*d1 + d1*d2 + d2*d2 + d1 + d2 + 1]) = G11 | P | G22 | global means | N; flags as above.
+template <typename T>
+size_t ccaloss_fwd_moments_workspace_bytes(const ColumnLayout& L);
+template <typename T>
+int ccaloss_forward_moments(const ColumnLayout& L, const double* moments, const double* n_dev, double eps, T* loss,
+                            T* saved, int* flags_out, void* ws, size_t ws_bytes, cudaStream_t stream);
+// This shard's rows (n >= 0) of dL/dz of the global loss: g1 <- 2/(N-1) (z1 G11 - z2 P^T - 1 r_1^T) grad_out[0] with
+// r_1 = mu_1^T G11 - mu_2^T P^T from the saved global means, g2 symmetric.  No collective.
+template <typename T>
+int ccaloss_backward_global(int d1, int d2, const T* z1, int64_t ld1, const T* z2, int64_t ld2, int64_t n,
+                            const T* saved, const T* grad_out, T* g1, int64_t ldg1, T* g2, int64_t ldg2,
+                            cudaStream_t stream);
+
 }  // namespace ccab

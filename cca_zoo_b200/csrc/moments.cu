@@ -824,9 +824,12 @@ __device__ __forceinline__ int compact_to_padded(const CovParams& p, int g) {
   return p.poff[v] + (g - p.coff[v]);
 }
 
-template <typename Tout>
-__global__ void covariance_kernel(const CovParams p, const double* __restrict__ mom, double n_total,
-                                  int center, Tout* __restrict__ C, int64_t ldc, Tout* __restrict__ mean) {
+// kDevN: the sample count is read at n_dev[0] (an all-reduced count that never left the device) instead of n_host
+template <typename Tout, bool kDevN>
+__global__ void covariance_kernel(const CovParams p, const double* __restrict__ mom, double n_host,
+                                  const double* __restrict__ n_dev, int center, Tout* __restrict__ C, int64_t ldc,
+                                  Tout* __restrict__ mean) {
+  const double n_total = kDevN ? n_dev[0] : n_host;
   const double* M = mom;
   const double* s = mom + (size_t)p.Dp * p.Dp;
   const int gi = blockIdx.y * blockDim.y + threadIdx.y;
@@ -1448,10 +1451,10 @@ int moments_unpack(const ColumnLayout& L, const double* packed, double* mom, cud
   return 0;
 }
 
-template <typename Tout>
-int covariance_from_moments(const ColumnLayout& L, const double* moments, double n_total, int center, Tout* C,
-                            int64_t ldc, Tout* mean, cudaStream_t stream) {
-  CCAB_CHECK_ARG(n_total >= 2.0, "need at least 2 samples for a covariance, got %g", n_total);
+namespace {
+template <typename Tout, bool kDevN>
+int launch_covariance(const ColumnLayout& L, const double* moments, double n_total, const double* n_dev, int center,
+                      Tout* C, int64_t ldc, Tout* mean, cudaStream_t stream) {
   CCAB_CHECK_ARG(ldc >= L.D, "ldc too small");
   CovParams p;
   p.n_views = L.n_views;
@@ -1464,14 +1467,34 @@ int covariance_from_moments(const ColumnLayout& L, const double* moments, double
   }
   dim3 block(32, 8);
   dim3 grid((unsigned)ceil_div(L.D, 32), (unsigned)ceil_div(L.D, 8));
-  covariance_kernel<Tout><<<grid, block, 0, stream>>>(p, moments, n_total, center, C, ldc, mean); count_launches(1);
+  covariance_kernel<Tout, kDevN><<<grid, block, 0, stream>>>(p, moments, n_total, n_dev, center, C, ldc, mean);
+  count_launches(1);
   CCAB_CUDA(cudaGetLastError());
   return 0;
+}
+}  // namespace
+
+template <typename Tout>
+int covariance_from_moments(const ColumnLayout& L, const double* moments, double n_total, int center, Tout* C,
+                            int64_t ldc, Tout* mean, cudaStream_t stream) {
+  CCAB_CHECK_ARG(n_total >= 2.0, "need at least 2 samples for a covariance, got %g", n_total);
+  return launch_covariance<Tout, false>(L, moments, n_total, nullptr, center, C, ldc, mean, stream);
+}
+
+template <typename Tout>
+int covariance_from_moments_ndev(const ColumnLayout& L, const double* moments, const double* n_dev, int center,
+                                 Tout* C, int64_t ldc, Tout* mean, cudaStream_t stream) {
+  CCAB_CHECK_ARG(n_dev != nullptr, "n_dev is NULL");
+  return launch_covariance<Tout, true>(L, moments, 0.0, n_dev, center, C, ldc, mean, stream);
 }
 
 template int covariance_from_moments<float>(const ColumnLayout&, const double*, double, int, float*, int64_t, float*,
                                             cudaStream_t);
 template int covariance_from_moments<double>(const ColumnLayout&, const double*, double, int, double*, int64_t,
                                              double*, cudaStream_t);
+template int covariance_from_moments_ndev<float>(const ColumnLayout&, const double*, const double*, int, float*,
+                                                 int64_t, float*, cudaStream_t);
+template int covariance_from_moments_ndev<double>(const ColumnLayout&, const double*, const double*, int, double*,
+                                                  int64_t, double*, cudaStream_t);
 
 }  // namespace ccab

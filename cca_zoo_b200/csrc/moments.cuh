@@ -40,6 +40,10 @@ int moments_simt(const ColumnLayout& L, const void* const* views, const int64_t*
 template <typename Tout>
 int covariance_from_moments(const ColumnLayout& L, const double* moments, double n_total, int center,
                             Tout* C, int64_t ldc, Tout* mean, cudaStream_t stream);
+// the same with the sample count read at n_dev[0] on the device (an all-reduced count; N < 2 gives inf / NaN entries)
+template <typename Tout>
+int covariance_from_moments_ndev(const ColumnLayout& L, const double* moments, const double* n_dev, int center,
+                                 Tout* C, int64_t ldc, Tout* mean, cudaStream_t stream);
 
 // exchange-step message: upper triangle of 128 x 128 blocks | column sums | n | reserved (all float64)
 int64_t moments_packed_size(const ColumnLayout& L);

@@ -15,13 +15,21 @@ Forward  : ONE library call (``ccab_ccaloss_fwd``, csrc/fit.cu): moment pass ove
            ``clamp(eigh(S + eps I), min=eps)`` literally with two Jacobi eigendecompositions.
 Backward : analytic (SURVEY.md §3.4), no eigh-backward, ONE library call (``ccab_ccaloss_bwd``): with
            P = S11^-1 S12 S22^-1,  dL/dz1 = 2/(n-1) * center(z1 (P S21 S11^-1) - z2 P^T),  dL/dz2 symmetric.
+
+Global batch (``global_batch=True`` under data parallelism, CCALoss / MCCALoss / GCCALoss): each rank's moment buffer
+is summed over the ranks with ONE exchange (``parallel.allreduce_moments_lazy``, the step of the sharded fit), and the
+loss stage runs on the global moments with the global count N read on the device (``ccab_ccaloss_fwd_moments``,
+``ccab_covariance_ndev``).  The loss is the loss of the concatenated global batch, replicated on every rank; each rank's
+backward is the exact derivative of that loss with respect to its own rows, centred by the saved global means, with no
+collective (``ccab_ccaloss_bwd_global``, ``ccab_row_sub_scale``).  Every route decision is taken from exchanged data, so
+all ranks take the same route and raise at the same call.
 """
 from __future__ import annotations
 
 import torch
 import torch.nn as nn
 
-from .. import ops
+from .. import ops, parallel
 
 
 def _require_cuda(name, *tensors):
@@ -101,6 +109,12 @@ def _eigen_route(z1d, z2d, eps, precision):
     n, d1 = z1d.shape[0], z1d.shape[1]
     mom = ops.moments([z1d, z2d], precision=precision)
     C, _ = ops.covariance(mom, [d1, z2d.shape[1]], n, center=True, dtype=z1d.dtype)
+    means = torch.cat([z1d.mean(dim=0), z2d.mean(dim=0)])     # the fused narrow backward centres algebraically
+    return _eigen_stage(C, d1, eps, means)
+
+
+def _eigen_stage(C, d1, eps, means):
+    """The eigen route from the block covariance C of [z1 z2]: (loss, saved = G11 | P | G22 | means)."""
     S12 = C[:d1, d1:].contiguous()
     whiten = []
     for blk in (C[:d1, :d1], C[d1:, d1:]):
@@ -116,9 +130,54 @@ def _eigen_route(z1d, z2d, eps, precision):
     P = ops.gemm(ops.gemm(S1inv, S12), S2inv)
     g11 = ops.gemm(ops.gemm(P, S12, transb=True), S1inv)
     g22 = ops.gemm(ops.gemm(S2inv, S12, transb=True), P)
-    means = torch.cat([z1d.mean(dim=0), z2d.mean(dim=0)])     # the fused narrow backward centres algebraically
     saved = torch.cat([g11.reshape(-1), P.reshape(-1), g22.reshape(-1), means])
     return loss, saved
+
+
+def _is_global(global_batch, group):
+    """Global-batch statistics apply only with more than one rank; otherwise the per-replica route runs unchanged."""
+    return bool(global_batch) and parallel.is_distributed(group)
+
+
+def _exchange(zd, precision, group):
+    """The ONE collective of a global-batch forward: this rank's moment buffer summed over the ranks.  Returns
+    (moments of the global batch, N as a 1-element float64 device tensor) -- nothing is read back."""
+    dims = [int(z.shape[1]) for z in zd]
+    n_local = int(zd[0].shape[0])
+    if n_local > 0:
+        mom = ops.moments(zd, precision=precision)
+    else:   # no rows here: contribute zeros (raising would leave the other ranks waiting in the exchange)
+        mom = torch.zeros(ops.moments_size(dims), dtype=torch.float64, device=zd[0].device)
+    mom, _, n_dev = parallel.allreduce_moments_lazy(mom, n_local, group, dims)
+    return mom, n_dev
+
+
+def _global_count(n_dev, what):
+    """N on the host (one read-back, taken only where the route depends on it)."""
+    N = int(round(float(n_dev.reshape(-1)[0].item())))
+    if N < 2:
+        raise ValueError(f"{what}: a global batch needs at least 2 samples over all ranks, got N = {N}.")
+    return N
+
+
+def _check_finite(C, what):
+    if not bool(torch.isfinite(C).all()):          # only on routes that read back anyway
+        raise ValueError(f"{what}: a representation contained NaN or infinity.")
+
+
+def _eigen_route_global(mom, n_dev, d1, d2, eps, dtype):
+    """The eigen route from the global moments: (loss, saved = G11 | P | G22 | global means | N)."""
+    _global_count(n_dev, "CCALoss")
+    C, mean = ops.covariance(mom, [d1, d2], n_dev, center=True, dtype=dtype)
+    _check_finite(C, "CCALoss")
+    loss, saved = _eigen_stage(C, d1, eps, mean)
+    return loss, torch.cat([saved, n_dev.to(dtype).reshape(1)])
+
+
+def _check_pair(z1, z2, name):
+    _require_cuda(name, z1, z2)
+    if z1.dtype != z2.dtype or z1.dtype not in (torch.float32, torch.float64):
+        raise ValueError("representations must share a float32/float64 dtype")
 
 
 class _CCALossFn(torch.autograd.Function):
@@ -153,6 +212,41 @@ class _CCALossFn(torch.autograd.Function):
         return g1, g2, None, None, None, None
 
 
+class _CCALossGlobalFn(torch.autograd.Function):
+    """CCALoss of the global batch: this rank's rows, the moments of all ranks (see the module docstring)."""
+
+    @staticmethod
+    def forward(ctx, z1, z2, eps, precision, status, sync, group):
+        _check_pair(z1, z2, "CCALoss")
+        n, d1, d2 = int(z1.shape[0]), int(z1.shape[1]), int(z2.shape[1])
+        z1d, z2d = _row_major(z1), _row_major(z2)
+        mom, n_dev = _exchange([z1d, z2d], _resolve_precision(precision, [z1d, z2d]), group)
+        width = max(d1, d2)
+        # n - 1 >= width here implies N - 1 >= width: no read-back.  Only a narrower shard reads N, and N (exchanged)
+        # decides for every rank alike.
+        eigen = n - 1 < width and _global_count(n_dev, "CCALoss") - 1 < width
+        if not eigen:
+            loss, saved, flags = ops.ccaloss_fwd_moments(mom, n_dev, d1, d2, eps, z1.dtype)
+            if sync:
+                f = flags.tolist()                            # flags of the global moments: the same on every rank
+                if f[2]:
+                    raise ValueError("CCALoss: a representation contained NaN or infinity.")
+                eigen = bool(f[0] or f[1])
+            else:
+                status.push(flags)
+        if eigen:
+            loss, saved = _eigen_route_global(mom, n_dev, d1, d2, eps, z1.dtype)
+        ctx.save_for_backward(z1d, z2d, saved)
+        return loss.reshape(()).clone()
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        z1, z2, saved = ctx.saved_tensors
+        go = grad_out.to(z1.dtype).reshape(1).contiguous()
+        g1, g2 = ops.ccaloss_bwd_global(z1, z2, saved, go)
+        return g1, g2, None, None, None, None, None
+
+
 class CCALoss(nn.Module):
     r"""Andrew et al. (2013) deep-CCA loss for two views (cca_zoo/deep/objectives.py:24-102).
 
@@ -164,15 +258,27 @@ class CCALoss(nn.Module):
             evaluation is copied to the host asynchronously and inspected at the next call / by ``check()``, which
             raise if an earlier batch had a numerically indefinite covariance.  ``"sync"`` reads the status back in
             every call and takes the eigen route (the reference's ``clamp(eigh(.))`` literally) for such batches.
+        global_batch: under data parallelism (an initialised process group of more than one rank), compute the loss
+            of the concatenated global batch instead of each replica's own: the block moments are summed over the
+            ranks with one exchange per forward, every rank gets the same loss, and each rank's backward (no
+            collective) is the exact derivative of that loss with respect to its own rows.  A rank may hold 0 rows.
+            DDP averages parameter gradients over the W ranks, so they come out as (1/W) dL_global/dθ.  Without a
+            process group, or with one rank, the per-replica route runs unchanged.  Default False (the reference's
+            per-replica statistics).
+        process_group: the ranks whose batches form the global batch (``None``: the default group, as in
+            ``torch.nn.SyncBatchNorm``).
     """
 
-    def __init__(self, eps: float = 1e-5, precision: str = "auto", verify: str = "lazy") -> None:
+    def __init__(self, eps: float = 1e-5, precision: str = "auto", verify: str = "lazy", global_batch: bool = False,
+                 process_group=None) -> None:
         super().__init__()
         if verify not in ("lazy", "sync"):
             raise ValueError("verify must be 'lazy' or 'sync'")
         self.eps = eps
         self.precision = precision
         self.verify = verify
+        self.global_batch = global_batch
+        self.process_group = process_group
         self._status = _LazyStatus("CCALoss")
 
     def check(self) -> None:
@@ -187,7 +293,85 @@ class CCALoss(nn.Module):
             )
         self._status.poll()
         z1, z2 = representations
+        if _is_global(self.global_batch, self.process_group):
+            return _CCALossGlobalFn.apply(z1, z2, float(self.eps), self.precision, self._status, self.verify == "sync",
+                                          self.process_group)
         return _CCALossFn.apply(z1, z2, float(self.eps), self.precision, self._status, self.verify == "sync")
+
+
+def _mcca_cholesky_inverses(C, off, dims, eps):
+    """A_i = (C_ii + eps I)^-1 by batched Cholesky + inverse; returns (A, Cholesky status tensors)."""
+    m = len(dims)
+    A, flags = [], []
+    if len(set(dims)) == 1:                                  # one batched factorisation for all views
+        R = torch.stack([C[off[i]:off[i + 1], off[i]:off[i + 1]] for i in range(m)])
+        R.diagonal(dim1=1, dim2=2).add_(eps)
+        Linv, info = ops.potrf_inv_(R, pivot_tol=0.25 * eps)
+        flags.append(info)
+        Ab = ops.gemm_batched(Linv, Linv, transa=True)
+        A = [Ab[i] for i in range(m)]
+    else:
+        for i in range(m):
+            R = C[off[i]:off[i + 1], off[i]:off[i + 1]].contiguous()
+            R.diagonal().add_(eps)
+            Linv, info = ops.potrf_inv_(R, pivot_tol=0.25 * eps)
+            flags.append(info)
+            A.append(ops.gemm(Linv, Linv, transa=True))
+    return A, flags
+
+
+def _mcca_eigen_inverses(C, off, dims, eps):
+    """A_i = clamp(eigh(C_ii + eps I), min=eps)^-1 = W_i^T W_i, the inverse each pair's eigen route uses; returns the
+    A_i and the whitening rows W_i."""
+    A, W = [], []
+    for i in range(len(dims)):
+        lam, Vt = ops.syevj(C[off[i]:off[i + 1], off[i]:off[i + 1]].contiguous())
+        Wt, _, _ = ops.whiten_rows(lam, Vt, 0.0, floor_add=eps, rank_tol=-1.0, lam_floor=0.0)
+        A.append(ops.gemm(Wt, Wt, transa=True))
+        W.append(Wt)
+    return A, W
+
+
+def _mcca_pairs(C, off, dims, A, W=None):
+    """P_ij = A_i S_ij A_j, G_i = sum_j P_ij S_ji A_i and the loss terms <P_ij, S_ij> over the pairs i < j.  With the
+    whitening rows W of the eigen route the terms are ||W_i S_ij W_j^T||_F^2 instead, as in CCALoss's eigen route: the
+    same value, without the cancellation of the trace form when a clamped eigenvalue makes A_i huge."""
+    m, dt = len(dims), C.dtype
+    G = [torch.zeros((d, d), dtype=dt, device=C.device) for d in dims]
+    P = {}
+    terms = []
+    for i in range(m):
+        for j in range(i + 1, m):
+            Sij = C[off[i]:off[i + 1], off[j]:off[j + 1]]
+            Q = ops.gemm(A[i], Sij)                          # A_i S_ij
+            Q2 = ops.gemm(Sij, A[j])                         # S_ij A_j
+            Pij = ops.gemm(Q, A[j])
+            ops.gemm(Pij, Q, transb=True, beta=1.0, out=G[i])            # += P_ij S_ji A_i
+            ops.gemm(Q2, Pij, transa=True, beta=1.0, out=G[j])           # += A_j S_ji P_ij
+            P[(i, j)] = Pij
+            if W is None:
+                terms.append((Pij * Sij).sum())
+            else:
+                f = ops.frobenius_norm(ops.gemm(ops.gemm(W[i], Sij), W[j], transb=True))
+                terms.append((f * f).reshape(()))
+    return G, P, terms
+
+
+def _mcca_products(xs, G, P, alpha):
+    """x_i G_i - sum_{j != i} x_j P_ji for every view (alpha times), x_i = z_i rows or a mean row."""
+    m = len(xs)
+    out = []
+    for i in range(m):
+        g = ops.gemm(xs[i], G[i], alpha=alpha)
+        for j in range(m):
+            if j == i:
+                continue
+            if i < j:
+                ops.gemm(xs[j], P[(i, j)], transb=True, alpha=-alpha, beta=1.0, out=g)   # - x_j P_ij^T
+            else:
+                ops.gemm(xs[j], P[(j, i)], alpha=-alpha, beta=1.0, out=g)                # - x_j P_ji
+        out.append(g)
+    return out
 
 
 class _MCCALossFn(torch.autograd.Function):
@@ -212,35 +396,8 @@ class _MCCALossFn(torch.autograd.Function):
             off.append(off[-1] + d)
         mom = ops.moments(zd, precision=_resolve_precision(precision, zd))
         C, _ = ops.covariance(mom, dims, n, center=True, dtype=dt)
-        A, flags = [], []
-        if len(set(dims)) == 1:                                  # one batched factorisation for all views
-            d = dims[0]
-            R = torch.stack([C[off[i]:off[i + 1], off[i]:off[i + 1]] for i in range(m)])
-            R.diagonal(dim1=1, dim2=2).add_(eps)
-            Linv, info = ops.potrf_inv_(R, pivot_tol=0.25 * eps)
-            flags.append(info)
-            Ab = ops.gemm_batched(Linv, Linv, transa=True)
-            A = [Ab[i] for i in range(m)]
-        else:
-            for i in range(m):
-                R = C[off[i]:off[i + 1], off[i]:off[i + 1]].contiguous()
-                R.diagonal().add_(eps)
-                Linv, info = ops.potrf_inv_(R, pivot_tol=0.25 * eps)
-                flags.append(info)
-                A.append(ops.gemm(Linv, Linv, transa=True))
-        G = [torch.zeros((d, d), dtype=dt, device=C.device) for d in dims]
-        P = {}
-        terms = []
-        for i in range(m):
-            for j in range(i + 1, m):
-                Sij = C[off[i]:off[i + 1], off[j]:off[j + 1]]
-                Q = ops.gemm(A[i], Sij)                          # A_i S_ij
-                Q2 = ops.gemm(Sij, A[j])                         # S_ij A_j
-                Pij = ops.gemm(Q, A[j])
-                ops.gemm(Pij, Q, transb=True, beta=1.0, out=G[i])            # += P_ij S_ji A_i
-                ops.gemm(Q2, Pij, transa=True, beta=1.0, out=G[j])           # += A_j S_ji P_ij
-                P[(i, j)] = Pij
-                terms.append((Pij * Sij).sum())
+        A, flags = _mcca_cholesky_inverses(C, off, dims, eps)
+        G, P, terms = _mcca_pairs(C, off, dims, A)
         status.push(torch.cat(flags))
         ctx.n, ctx.m = n, m
         ctx.pairs = sorted(P)
@@ -270,27 +427,103 @@ class _MCCALossFn(torch.autograd.Function):
         return (None, None, None, *grads)
 
 
+class _MCCALossGlobalFn(torch.autograd.Function):
+    """MCCALoss of the global batch: one exchange, the pairs from the global C; backward with the global means."""
+
+    @staticmethod
+    def forward(ctx, eps, precision, status, sync, group, *zs):
+        _require_cuda("MCCALoss", *zs)
+        dt = zs[0].dtype
+        if dt not in (torch.float32, torch.float64) or any(z.dtype != dt for z in zs):
+            raise ValueError("representations must share a float32/float64 dtype")
+        n, m = int(zs[0].shape[0]), len(zs)
+        zd = [_row_major(z) for z in zs]
+        dims = [int(z.shape[1]) for z in zd]
+        off = [0]
+        for d in dims:
+            off.append(off[-1] + d)
+        mom, n_dev = _exchange(zd, _resolve_precision(precision, zd), group)
+        C, mean = ops.covariance(mom, dims, n_dev, center=True, dtype=dt)
+        eigen = n - 1 < max(dims) and _global_count(n_dev, "MCCALoss") - 1 < max(dims)
+        W = None                                   # whitening rows, on the eigen route only
+        if not eigen:
+            A, flags = _mcca_cholesky_inverses(C, off, dims, eps)
+            flags = torch.cat(flags + [(~torch.isfinite(C).all()).to(torch.int32).reshape(1)])
+            if sync:
+                f = flags.tolist()                 # from the global C: the same on every rank
+                if f[-1]:
+                    raise ValueError("MCCALoss: a representation contained NaN or infinity.")
+                eigen = any(f[:-1])
+            else:
+                status.push(flags)
+        if eigen:                                  # every pair through the eigen route, from the same global C
+            _global_count(n_dev, "MCCALoss")
+            _check_finite(C, "MCCALoss")
+            A, W = _mcca_eigen_inverses(C, off, dims, eps)
+        G, P, terms = _mcca_pairs(C, off, dims, A, W)
+        ctx.m = m
+        ctx.pairs = sorted(P)
+        ctx.save_for_backward(mean, n_dev, *zd, *G, *[P[k] for k in ctx.pairs])
+        return -torch.stack(terms).sum()
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        m = ctx.m
+        mean, n_dev, *t = ctx.saved_tensors
+        zs, G = t[:m], t[m:2 * m]
+        P = dict(zip(ctx.pairs, t[2 * m:]))
+        dt = zs[0].dtype
+        # dL/dz_i = 2/(N-1) (z_i G_i - sum_j z_j P_ji - 1 r_i^T) go, r_i the same product of the global mean rows
+        s = (2.0 / (n_dev - 1.0)).to(dt) * grad_out.to(dt).reshape(1)
+        mus, o = [], 0
+        for z in zs:
+            mus.append(mean[o:o + z.shape[1]].reshape(1, -1))
+            o += z.shape[1]
+        if zs[0].shape[0] == 0:
+            return (None, None, None, None, None, *[torch.zeros_like(z) for z in zs])
+        rows = _mcca_products(mus, G, P, 1.0)
+        grads = _mcca_products(list(zs), G, P, 1.0)
+        for g, r in zip(grads, rows):
+            ops.row_sub_scale_(g, r.reshape(-1), s)
+        return (None, None, None, None, None, *grads)
+
+
 class MCCALoss(nn.Module):
     r"""Sum of pairwise CCA losses over all view pairs (cca_zoo/deep/objectives.py:105-153), computed from one
     moment pass with every within-view covariance factored once.  Same ``verify`` semantics as ``CCALoss``
     (``"lazy"``: status checked at the next call; ``"sync"``: per-pair ``CCALoss`` evaluations with the eigen-route
-    fallback, i.e. the reference's loop)."""
+    fallback, i.e. the reference's loop).
 
-    def __init__(self, eps: float = 1e-5, precision: str = "auto", verify: str = "lazy") -> None:
+    ``global_batch`` / ``process_group`` as in ``CCALoss`` (2 to 8 views): one exchange per forward, and all pairs come
+    from the global block covariance.  There ``verify="sync"`` reads the replicated status and, if some S_ii failed,
+    evaluates every pair through the eigen route from the same global covariance (no per-pair exchanges)."""
+
+    def __init__(self, eps: float = 1e-5, precision: str = "auto", verify: str = "lazy", global_batch: bool = False,
+                 process_group=None) -> None:
         super().__init__()
         if verify not in ("lazy", "sync"):
             raise ValueError("verify must be 'lazy' or 'sync'")
         self.eps = eps
         self.precision = precision
         self.verify = verify
+        self.global_batch = global_batch
+        self.process_group = process_group
         self._status = _LazyStatus("MCCALoss", nan_last=False)
+        self._global_status = _LazyStatus("MCCALoss")
         self._cca_loss = CCALoss(eps=eps, precision=precision, verify="sync")
 
     def check(self) -> None:
         self._status.check()
+        self._global_status.check()
 
     def forward(self, representations: list[torch.Tensor]) -> torch.Tensor:
         n_views = len(representations)
+        if _is_global(self.global_batch, self.process_group):
+            if not 2 <= n_views <= 8:
+                raise ValueError(f"MCCALoss with global_batch=True takes 2 to 8 representations, got {n_views}.")
+            self._global_status.poll()
+            return _MCCALossGlobalFn.apply(float(self.eps), self.precision, self._global_status, self.verify == "sync",
+                                           self.process_group, *representations)
         n = representations[0].shape[0]
         lazy_ok = (self.verify == "lazy" and 2 <= n_views <= 8
                    and n - 1 >= max(int(z.shape[1]) for z in representations))
@@ -317,7 +550,7 @@ class _GCCALossFn(torch.autograd.Function):
     """
 
     @staticmethod
-    def forward(ctx, eps, precision, *zs):
+    def forward(ctx, eps, precision, glob, group, *zs):
         _require_cuda("GCCALoss", *zs)
         dt = zs[0].dtype
         if dt not in (torch.float32, torch.float64) or any(z.dtype != dt for z in zs):
@@ -326,8 +559,16 @@ class _GCCALossFn(torch.autograd.Function):
         dims = [int(z.shape[1]) for z in zs]
         D, k = sum(dims), dims[0]
         zd = [z.detach() for z in zs]
-        mom = ops.moments(zd, precision=precision)
-        C, _ = ops.covariance(mom, dims, n, center=True, dtype=dt)
+        mean = None
+        if glob:
+            # global batch: one exchange; N is read back (the Jacobi sweeps below read back anyway) and replaces n
+            mom, n_dev = _exchange(zd, precision, group)
+            C, mean = ops.covariance(mom, dims, n_dev, center=True, dtype=dt)
+            n = _global_count(n_dev, "GCCALoss")
+            _check_finite(C, "GCCALoss")
+        else:
+            mom = ops.moments(zd, precision=precision)
+            C, _ = ops.covariance(mom, dims, n, center=True, dtype=dt)
         Wt = torch.zeros((D, D), dtype=dt, device=C.device)
         off = 0
         for d in dims:
@@ -339,13 +580,13 @@ class _GCCALossFn(torch.autograd.Function):
         K = 0.5 * (K + K.T)
         evals, Ut = ops.syevj(K)                              # descending; rows of Ut are eigenvectors
         lam_k = evals[:k].contiguous()
-        ctx.n, ctx.dims = n, dims
-        ctx.save_for_backward(C, Wt, lam_k, Ut[:k].contiguous(), *zd)
+        ctx.n, ctx.dims, ctx.glob = n, dims, glob
+        ctx.save_for_backward(C, Wt, lam_k, Ut[:k].contiguous(), mean, *zd)
         return -lam_k.sum()
 
     @staticmethod
     def backward(ctx, grad_out):
-        C, Wt, lam_k, Ut_k, *zs = ctx.saved_tensors
+        C, Wt, lam_k, Ut_k, mean, *zs = ctx.saved_tensors
         n, dims = ctx.n, ctx.dims
         k = lam_k.shape[0]
         safe = lam_k.clamp_min(torch.finfo(lam_k.dtype).tiny * 1e8)
@@ -353,6 +594,8 @@ class _GCCALossFn(torch.autograd.Function):
         Q = ops.gemm(Wt, Qt, transa=True, transb=True)                    # D x k
         A = ops.gemm(C, Q, alpha=float(n - 1))                            # D x k
         B = ops.gemm(Wt, ops.gemm(Wt, A), transa=True)                    # blkdiag(S_i^-1) A
+        if ctx.glob:
+            return (None, None, None, None, *_gcca_global_grads(zs, dims, Q, B, mean, n, grad_out))
         Y = torch.zeros((n, k), dtype=C.dtype, device=C.device)
         off = 0
         for z, d in zip(zs, dims):
@@ -367,23 +610,63 @@ class _GCCALossFn(torch.autograd.Function):
             ops.center_columns_(g)
             grads.append(g * go)
             off += d
-        return (None, None, *grads)
+        return (None, None, None, None, *grads)
+
+
+def _gcca_global_grads(zs, dims, Q, B, mean, N, grad_out):
+    """This shard's rows of the global GCCA gradient: the local products, centred by the same products of the global
+    mean row, times grad_out -- no collective."""
+    dt = Q.dtype
+
+    def products(xs):
+        Y = torch.zeros((xs[0].shape[0], Q.shape[1]), dtype=dt, device=Q.device)
+        off = 0
+        for x, d in zip(xs, dims):
+            ops.gemm(x, Q[off:off + d], beta=1.0, out=Y)
+            off += d
+        out, off = [], 0
+        for x, d in zip(xs, dims):
+            Bi = B[off:off + d]
+            g = ops.gemm(Y, Bi, transb=True, alpha=-2.0)
+            ops.gemm(x, ops.gemm(Bi, Bi, transb=True), alpha=2.0 / (N - 1), beta=1.0, out=g)
+            out.append(g)
+            off += d
+        return out
+
+    mus, off = [], 0
+    for d in dims:
+        mus.append(mean[off:off + d].reshape(1, d))
+        off += d
+    if zs[0].shape[0] == 0:
+        return [torch.zeros_like(z) for z in zs]
+    rows = products(mus)
+    go = grad_out.to(dt).reshape(1)
+    grads = products(list(zs))
+    for g, r in zip(grads, rows):
+        ops.row_sub_scale_(g, r.reshape(-1), go)
+    return grads
 
 
 class GCCALoss(nn.Module):
     r"""Generalised (MAX-VAR) CCA loss for two or more views (cca_zoo/deep/objectives.py:156-220):
     :math:`-\sum_{d \le k} \lambda_d(\sum_i H_i H_i^\top)` with ``k`` the width of the first representation.
     Same constructor and ``forward(list[Tensor]) -> 0-dim Tensor`` as the reference, so it plugs into
-    ``DCCA(objective=...)`` and is what ``DGCCA`` uses (cca_zoo/deep/_dgcca.py:70).  At most 8 views."""
+    ``DCCA(objective=...)`` and is what ``DGCCA`` uses (cca_zoo/deep/_dgcca.py:70).  At most 8 views.
+    ``global_batch`` / ``process_group`` as in ``CCALoss``: one exchange per forward, and the eigenproblem of the
+    global block covariance (its Jacobi sweeps read back, as the per-replica route's do, and so does N)."""
 
-    def __init__(self, eps: float = 1e-5, precision: str = "exact") -> None:
+    def __init__(self, eps: float = 1e-5, precision: str = "exact", global_batch: bool = False,
+                 process_group=None) -> None:
         super().__init__()
         self.eps = eps
         self.precision = precision
+        self.global_batch = global_batch
+        self.process_group = process_group
 
     def forward(self, representations: list[torch.Tensor]) -> torch.Tensor:
         prec = _resolve_precision(self.precision, [_row_major(z) for z in representations])
-        return _GCCALossFn.apply(float(self.eps), prec, *representations)
+        glob = _is_global(self.global_batch, self.process_group)
+        return _GCCALossFn.apply(float(self.eps), prec, glob, self.process_group if glob else None, *representations)
 
 
 def _tcca_divided_differences(lam, eps):

@@ -203,8 +203,17 @@ def moments_safe(views, precision: str = "tf32x3b", x0=None):
     return moments_unshift_(mom, [int(v.shape[1]) for v in views], x0, views[0].shape[0]), x0
 
 
-def covariance(mom: torch.Tensor, dims, n_total: float, center: bool = True, dtype=torch.float64):
-    """(C [D,D], mean [D]) from an (all-reduced) moments buffer."""
+def moments_size(dims) -> int:
+    """Entries of the moment buffer of views of widths ``dims`` (the zero buffer of a rank without rows)."""
+    size = _lib.load().ccab_moments_size(len(dims), _lib.i64_array(dims))
+    if size < 0:
+        raise ValueError(_lib.last_error())
+    return int(size)
+
+
+def covariance(mom: torch.Tensor, dims, n_total, center: bool = True, dtype=torch.float64):
+    """(C [D,D], mean [D]) from an (all-reduced) moments buffer.  ``n_total``: a number, or a 1-element float64 device
+    tensor (the count of an all-reduced buffer, read on the device: nothing is read back, and N < 2 is not refused)."""
     lib = _lib.load()
     _require_cuda(mom, "moments")
     D = int(sum(dims))
@@ -214,10 +223,19 @@ def covariance(mom: torch.Tensor, dims, n_total: float, center: bool = True, dty
     if mom.dtype != torch.float64 or mom.numel() != expect or not mom.is_contiguous():
         raise ValueError(f"moments buffer must be a contiguous float64 tensor of {expect} elements for widths "
                          f"{list(dims)}, got {mom.dtype} x {mom.numel()}")
-    if not n_total >= 2:
+    n_dev = n_total if isinstance(n_total, torch.Tensor) else None
+    if n_dev is not None and (n_dev.dtype != torch.float64 or n_dev.numel() != 1 or n_dev.device != mom.device):
+        raise ValueError("a device-side n_total must be a 1-element float64 tensor on the moments' device")
+    if n_dev is None and not n_total >= 2:
         raise ValueError(f"at least 2 samples are needed for a covariance, got n = {n_total}")
     Cm = torch.empty((D, D), dtype=dtype, device=mom.device)
     mean = torch.empty(D, dtype=dtype, device=mom.device)
+    if n_dev is not None:
+        with torch.cuda.device(mom.device):
+            rc = lib.ccab_covariance_ndev(_DT[dtype], len(dims), _lib.i64_array(dims), _ptr(mom), _ptr(n_dev),
+                                          1 if center else 0, _ptr(Cm), D, _ptr(mean), _stream(mom))
+        _lib.check(rc, "ccab_covariance_ndev")
+        return Cm, mean
     with torch.cuda.device(mom.device):
         rc = lib.ccab_covariance(_DT[dtype], len(dims), _lib.i64_array(dims), _ptr(mom), float(n_total),
                                  1 if center else 0, _ptr(Cm), D, _ptr(mean), _stream(mom))
@@ -473,6 +491,60 @@ def ccaloss_bwd(z1, z2, saved, grad_out):
                                   _ptr(grad_out), _ptr(g1), d1, _ptr(g2), d2, _stream(z1))
     _lib.check(rc, "ccab_ccaloss_bwd")
     return g1, g2
+
+
+def ccaloss_fwd_moments(mom, n_dev, d1, d2, eps, dtype):
+    """The deep-CCA objective of a global batch (ccab_ccaloss_fwd_moments): ``mom`` is the moment buffer of [z1 z2]
+    summed over the ranks, ``n_dev`` its 1-element float64 device count.  Returns (loss[1], saved, flags int32[3]), all
+    on the device; saved = G11 | P | G22 | global means | N."""
+    lib = _lib.load()
+    _require_cuda(mom, "moments")
+    _require_cuda(n_dev, "n_dev")
+    if mom.dtype != torch.float64 or not mom.is_contiguous() or mom.numel() != moments_size([d1, d2]):
+        raise ValueError(f"moments must be the contiguous float64 buffer of widths [{d1}, {d2}]")
+    if n_dev.dtype != torch.float64 or n_dev.numel() != 1:
+        raise ValueError("n_dev must be a 1-element float64 tensor")
+    loss = torch.empty(1, dtype=dtype, device=mom.device)
+    saved = torch.empty(d1 * d1 + d1 * d2 + d2 * d2 + d1 + d2 + 1, dtype=dtype, device=mom.device)
+    flags = torch.empty(3, dtype=torch.int32, device=mom.device)
+    ws = _ws(lib.ccab_ccaloss_fwd_moments_workspace_bytes(_DT[dtype], d1, d2), mom.device)
+    with torch.cuda.device(mom.device):
+        rc = lib.ccab_ccaloss_fwd_moments(_DT[dtype], d1, d2, _ptr(mom), _ptr(n_dev), float(eps), _ptr(loss),
+                                          _ptr(saved), _ptr(flags), _ptr(ws), ws.numel(), _stream(mom))
+    _lib.check(rc, "ccab_ccaloss_fwd_moments")
+    return loss, saved, flags
+
+
+def ccaloss_bwd_global(z1, z2, saved, grad_out):
+    """This shard's rows of the gradient of a global-batch deep-CCA loss (ccab_ccaloss_bwd_global), scaled by
+    grad_out; ``saved`` from ``ccaloss_fwd_moments`` (or the eigen route).  No collective, nothing read back."""
+    lib = _lib.load()
+    n, d1, d2 = z1.shape[0], z1.shape[1], z2.shape[1]
+    if saved.numel() != d1 * d1 + d1 * d2 + d2 * d2 + d1 + d2 + 1:
+        raise ValueError("saved does not come from a global-batch forward of these widths")
+    g1 = torch.empty((n, d1), dtype=z1.dtype, device=z1.device)
+    g2 = torch.empty((n, d2), dtype=z1.dtype, device=z1.device)
+    with torch.cuda.device(z1.device):
+        rc = lib.ccab_ccaloss_bwd_global(_DT[z1.dtype], _ptr(z1), max(z1.stride(0), d1), _ptr(z2),
+                                         max(z2.stride(0), d2), n, d1, d2, _ptr(saved), _ptr(grad_out), _ptr(g1), d1,
+                                         _ptr(g2), d2, _stream(z1))
+    _lib.check(rc, "ccab_ccaloss_bwd_global")
+    return g1, g2
+
+
+def row_sub_scale_(A, r, s):
+    """In place A[i, :] = (A[i, :] - r) * s[0] (ccab_row_sub_scale); r (n,) and s (1,) device tensors."""
+    lib = _lib.load()
+    _require_cuda(A, "A")
+    if A.dim() != 2 or A.stride(1) != 1 or r.numel() != A.shape[1] or s.numel() != 1:
+        raise ValueError("row_sub_scale_: a row-major (m, n) matrix, an n-vector r and a scalar s")
+    r = r.to(A.dtype).contiguous()
+    s = s.to(A.dtype).contiguous()
+    with torch.cuda.device(A.device):
+        rc = lib.ccab_row_sub_scale(_DT[A.dtype], A.shape[0], A.shape[1], _ptr(A), max(A.stride(0), A.shape[1]),
+                                    _ptr(r), _ptr(s), _stream(A))
+    _lib.check(rc, "ccab_row_sub_scale")
+    return A
 
 
 def potrf_inv_(A, pivot_tol=0.0):

@@ -112,6 +112,10 @@ int ccab_moments_exchange_nvls(int n_views, const int64_t* dims, double* moments
  * Replaces: the centring of cca_zoo/_base.py:96-99 plus the 1/(n-1) scalings listed above. */
 int ccab_covariance(int out_dtype, int n_views, const int64_t* dims, const double* moments, double n_total,
                     int center, void* C, int64_t ldc, void* mean, void* stream);
+/* The same with n_total read at n_dev[0] (device): the count of an all-reduced buffer needs no host read-back.
+ * N < 2 is not refused here (nothing is read back): C then holds inf / NaN. */
+int ccab_covariance_ndev(int out_dtype, int n_views, const int64_t* dims, const double* moments, const double* n_dev,
+                         int center, void* C, int64_t ldc, void* mean, void* stream);
 
 /* ---- K3: batched symmetric eigensolver (one-sided block Jacobi) ----------------------------------
  * For each of `batch` symmetric n x n matrices A_b (device, row-major == column-major, lda, stride
@@ -491,6 +495,22 @@ int ccab_ccaloss_bwd(int dtype, const void* z1, int64_t ld1, const void* z2, int
                      const void* saved, const void* grad_out, void* g1, int64_t ldg1, void* g2, int64_t ldg2,
                      void* stream);
 
+/* ---- the deep-CCA objective of a global batch (data-parallel ranks, moments all-reduced before the loss) ----------
+ * ccab_ccaloss_fwd_moments: the stage of ccab_ccaloss_fwd after its moment pass, from `moments` (the ccab_moments
+ * buffer of [z1 z2], summed over the ranks) with the sample count N read at n_dev[0] on the device.  Same loss and
+ * flags; `saved` (T[d1*d1 + d1*d2 + d2*d2 + d1 + d2 + 1]) = G11 | P | G22 | global column means of z1, z2 | N.
+ * ccab_ccaloss_bwd_global: this rank's n_local rows (0 allowed) of the gradient of the global loss,
+ *   g1 = 2/(N-1) (z1 G11 - z2 P^T - 1 (mu1^T G11 - mu2^T P^T)) * grad_out[0],  g2 symmetric,
+ * with mu and N from `saved`: 4 GEMMs over the local rows and one epilogue launch (widths <= 64: one fused launch).
+ * Neither reads anything back, and the backward needs nothing from the other ranks. */
+size_t ccab_ccaloss_fwd_moments_workspace_bytes(int dtype, int d1, int d2);
+int ccab_ccaloss_fwd_moments(int dtype, int d1, int d2, const double* moments, const double* n_dev, double eps,
+                             void* loss, void* saved, int* flags_dev, void* workspace, size_t workspace_bytes,
+                             void* stream);
+int ccab_ccaloss_bwd_global(int dtype, const void* z1, int64_t ld1, const void* z2, int64_t ld2, int64_t n_local, int d1,
+                            int d2, const void* saved, const void* grad_out, void* g1, int64_t ldg1, void* g2,
+                            int64_t ldg2, void* stream);
+
 /* B[i,j] = A[i,j] * f(r[i]) * f(c[j]); r / c may be NULL; *_pow: 0 -> x, 1 -> 1/x, 2 -> 1/sqrt(x).
  * (column scalings such as diag(sigma)^-1/2 in the GCCA back-substitution, cca_zoo/linear/_gcca.py:109) */
 int ccab_scale(int dtype, int m, int n, const void* A, int64_t lda, const void* r, int r_pow, const void* c,
@@ -498,6 +518,10 @@ int ccab_scale(int dtype, int m, int n, const void* A, int64_t lda, const void* 
 
 /* A[:, j] -= mean_i A[i, j] in place (the centring Jacobian of cca_zoo/deep/objectives.py:83-84) */
 int ccab_center_columns(int dtype, int m, int n, void* A, int64_t lda, void* stream);
+
+/* A[i, :] = (A[i, :] - r) * s[0] in place (m x n row-major; r: device T[n], s: device T[1]): the centring of a
+ * global-batch gradient by the all-reduced column means, with a scale that may depend on the device-side count */
+int ccab_row_sub_scale(int dtype, int64_t m, int n, void* A, int64_t lda, const void* r, const void* s, void* stream);
 
 /* out[0] (device) = ||A||_F of an m x n row-major matrix */
 int ccab_frobenius_norm(int dtype, int m, int n, const void* A, int64_t lda, void* out, void* stream);
