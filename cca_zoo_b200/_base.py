@@ -29,6 +29,7 @@ from sklearn.utils._param_validation import Interval, StrOptions
 from sklearn.utils.validation import check_is_fitted
 
 from . import ops, parallel
+from .ops import HALF_DTYPES
 from ._validation import validate_views
 
 
@@ -41,6 +42,19 @@ def _copy_stream(device):
     if key not in _COPY_STREAMS:
         _COPY_STREAMS[key] = torch.cuda.Stream(device)
     return _COPY_STREAMS[key]
+
+
+def _shared_half_dtype(views):
+    """The 16-bit dtype (torch.bfloat16 / torch.float16) all views share, else None.  numpy has no bfloat16; float16
+    arrays count as torch.float16."""
+    dts = {v.dtype if isinstance(v, torch.Tensor) else (torch.float16 if v.dtype == np.float16 else None)
+           for v in views}
+    dt = dts.pop() if len(dts) == 1 else None
+    return dt if dt in HALF_DTYPES else None
+
+
+def _as_tensor(v):
+    return v if isinstance(v, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(v))
 
 
 def _freeze(v):
@@ -142,25 +156,33 @@ class BaseModel(BaseEstimator, ABC):
     _stream_chunk_rows: ClassVar[int] = 16384
 
     def _local_moments(self, validated, device):
-        """Moment buffer of the rows this process holds.  Returns (moments, n_rows, dims, input dtype)."""
+        """Moment buffer of the rows this process holds.  Returns (moments, n_rows, dims, input dtype).
+
+        Views that share one 16-bit dtype (bfloat16 / float16 tensors, float16 arrays) reach the moment kernel as they
+        are, without a float64 copy; their input dtype is reported as float64, so every stage after the moment buffer
+        runs as it does for a float64 copy of them."""
+        half = _shared_half_dtype(validated)
         host = all(not (isinstance(v, torch.Tensor) and v.is_cuda) for v in validated)
         n_rows = int(validated[0].shape[0])
         nbytes = sum(int(np.prod(v.shape)) * (v.element_size() if isinstance(v, torch.Tensor) else v.dtype.itemsize)
                      for v in validated)
         if not (host and nbytes >= self._stream_threshold_bytes and n_rows >= 4 * self._stream_chunk_rows):
-            dev_views = [self._to_device(v, device) for v in validated]
-            if len({v.dtype for v in dev_views}) > 1:
-                dev_views = [v.to(torch.float64) for v in dev_views]
+            if half is not None:
+                dev_views = [_as_tensor(v).to(device, non_blocking=True) for v in validated]
+            else:
+                dev_views = [self._to_device(v, device) for v in validated]
+                if len({v.dtype for v in dev_views}) > 1:
+                    dev_views = [v.to(torch.float64) for v in dev_views]
             dims = [int(v.shape[1]) for v in dev_views]
             # shifted accumulation when a pilot over the leading rows finds badly centred columns (one-pass covariance
             # from raw moments would cancel: the reference centres first, cca_zoo/_base.py:96-99)
             mom, _ = ops.moments_safe(dev_views, precision=self.precision)
-            return mom, n_rows, dims, dev_views[0].dtype
+            return mom, n_rows, dims, torch.float64 if half is not None else dev_views[0].dtype
         # ---- streamed: the moments are additive over row chunks (the same identity the multi-GPU path uses) ----
         cpu_views = []
         for v in validated:
-            t = v if isinstance(v, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(v))
-            if t.dtype not in (torch.float32, torch.float64):
+            t = _as_tensor(v)
+            if t.dtype not in (torch.float32, torch.float64) and half is None:
                 t = t.to(torch.float64)
             cpu_views.append(t)
         if len({t.dtype for t in cpu_views}) > 1:
@@ -182,7 +204,7 @@ class BaseModel(BaseEstimator, ABC):
                 mom = self._accumulate(mom, pending, main)
             pending = (chunk, ready)
         mom = self._accumulate(mom, pending, main)
-        return mom, n_rows, dims, cpu_views[0].dtype
+        return mom, n_rows, dims, torch.float64 if half is not None else cpu_views[0].dtype
 
     def _accumulate(self, mom, pending, main):
         chunk, ready = pending

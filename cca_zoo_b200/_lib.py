@@ -12,7 +12,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libccab200.so")
 
-F32, F64 = 0, 1
+F32, F64, BF16, F16 = 0, 1, 2, 3   # BF16 / F16: the moments and the pilot / shift only
 PREC_TF32, PREC_TF32X3, PREC_EXACT, PREC_TF32X3B = 0, 1, 2, 3
 MAX_VIEWS = 8
 # metric ids of ccab_pairwise_kernel (CCAB_KERNEL_* in include/ccab200.h)

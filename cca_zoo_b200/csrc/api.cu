@@ -96,7 +96,8 @@ int ccab_moments(int dtype, int precision, int n_views, const void* const* views
                  const int64_t* lds, int64_t n_rows, double* moments, void* workspace, size_t workspace_bytes,
                  void* stream) {
   CCAB_TRY
-  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
+  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64 || dtype == CCAB_BF16 || dtype == CCAB_F16, "bad dtype %d",
+                 dtype);
   CCAB_CHECK_ARG(precision >= 0 && precision <= 3, "bad precision %d", precision);
   CCAB_CHECK_ARG(!(dtype == CCAB_F64 && precision != CCAB_PREC_EXACT),
                  "float64 inputs support CCAB_PREC_EXACT only (the TF32 tensor-core path has no f64 kind)");
@@ -113,9 +114,14 @@ int ccab_moments(int dtype, int precision, int n_views, const void* const* views
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (precision == CCAB_PREC_EXACT) {
     if (dtype == CCAB_F32) return moments_simt<float>(L, views, lds, n_rows, moments, workspace, workspace_bytes, s);
+    if (dtype == CCAB_BF16)
+      return moments_simt<__nv_bfloat16>(L, views, lds, n_rows, moments, workspace, workspace_bytes, s);
+    if (dtype == CCAB_F16) return moments_simt<__half>(L, views, lds, n_rows, moments, workspace, workspace_bytes, s);
     return moments_simt<double>(L, views, lds, n_rows, moments, workspace, workspace_bytes, s);
   }
-  return moments_tf32(L, views, lds, n_rows, precision, moments, workspace, workspace_bytes, s);
+  // every tensor precision of a 16-bit dtype is the 16-bit wgmma kernel: its products are exact, nothing to split
+  const int mode = dtype == CCAB_BF16 ? kModeBf16 : dtype == CCAB_F16 ? kModeF16 : precision;
+  return moments_tf32(L, views, lds, n_rows, mode, moments, workspace, workspace_bytes, s);
   CCAB_CATCH
 }
 
@@ -168,13 +174,19 @@ int ccab_moments_exchange_nvls(int n_views, const int64_t* dims, double* moments
 int ccab_column_pilot(int dtype, const void* X, int64_t rows, int d, int64_t ld, void* x0, float* ratio_max_dev,
                       void* stream) {
   CCAB_TRY
-  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
+  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64 || dtype == CCAB_BF16 || dtype == CCAB_F16, "bad dtype %d",
+                 dtype);
   CCAB_CHECK_ARG(X && x0 && ratio_max_dev, "null pointer argument");
   int rc = require_device();
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (dtype == CCAB_F32)
     return column_pilot<float>(static_cast<const float*>(X), rows, d, ld, static_cast<float*>(x0), ratio_max_dev, s);
+  if (dtype == CCAB_BF16)
+    return column_pilot<__nv_bfloat16>(static_cast<const __nv_bfloat16*>(X), rows, d, ld, static_cast<float*>(x0),
+                                       ratio_max_dev, s);
+  if (dtype == CCAB_F16)
+    return column_pilot<__half>(static_cast<const __half*>(X), rows, d, ld, static_cast<float*>(x0), ratio_max_dev, s);
   return column_pilot<double>(static_cast<const double*>(X), rows, d, ld, static_cast<double*>(x0), ratio_max_dev, s);
   CCAB_CATCH
 }
@@ -182,7 +194,8 @@ int ccab_column_pilot(int dtype, const void* X, int64_t rows, int d, int64_t ld,
 int ccab_shift_rows(int dtype, const void* X, int64_t n, int d, int64_t ldx, const void* x0, void* Xs, int64_t lds,
                     void* stream) {
   CCAB_TRY
-  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64, "bad dtype %d", dtype);
+  CCAB_CHECK_ARG(dtype == CCAB_F32 || dtype == CCAB_F64 || dtype == CCAB_BF16 || dtype == CCAB_F16, "bad dtype %d",
+                 dtype);
   CCAB_CHECK_ARG(X && x0 && Xs && ldx >= d && lds >= d, "bad argument");
   int rc = require_device();
   if (rc) return rc;
@@ -190,6 +203,12 @@ int ccab_shift_rows(int dtype, const void* X, int64_t n, int d, int64_t ldx, con
   if (dtype == CCAB_F32)
     return shift_rows<float>(static_cast<const float*>(X), n, d, ldx, static_cast<const float*>(x0),
                              static_cast<float*>(Xs), lds, s);
+  if (dtype == CCAB_BF16)
+    return shift_rows<__nv_bfloat16>(static_cast<const __nv_bfloat16*>(X), n, d, ldx, static_cast<const float*>(x0),
+                                     static_cast<float*>(Xs), lds, s);
+  if (dtype == CCAB_F16)
+    return shift_rows<__half>(static_cast<const __half*>(X), n, d, ldx, static_cast<const float*>(x0),
+                              static_cast<float*>(Xs), lds, s);
   return shift_rows<double>(static_cast<const double*>(X), n, d, ldx, static_cast<const double*>(x0),
                             static_cast<double*>(Xs), lds, s);
   CCAB_CATCH

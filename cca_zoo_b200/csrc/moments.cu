@@ -555,7 +555,168 @@ __global__ void __launch_bounds__(kPrThreads, 1) moments_x3b_pair_kernel(const _
 }
 
 // =============================================================================================
-// exact SIMT kernel (fp32 / fp64), 64x64 tiles inside the same padded tile space
+// 16-bit pair-tile kernel (bf16 / fp16 views)
+// =============================================================================================
+// The product of two bf16 or two fp16 values is exact in fp32 (8 + 8 and 11 + 11 significant bits), so one wgmma per
+// k16 step gives products as exact as the float64 route's: there is nothing to split.  wgmma reads 16-bit operands
+// MN-major from shared memory, so a TMA-loaded row-major slice of X is both operands as it lands: no transpose stage
+// and no register A path.
+// One CTA = one pair tile of moments_x3b_pair_kernel (A blocks 2i, 2i + 1 against a B block j >= 2i, the pair_tiles()
+// decode) over one split of the sample axis, computed transposed: MMA warpgroup g takes columns 64g .. 64g + 63 of B as
+// its M = 64 rows and the 256 columns of A0 | A1 as N, one m64n256k16 per k16 step (m64n128k16 against A0 alone when
+// j = 2i, whose A1 sub-tile lies below the block diagonal), and its epilogue writes the transpose into the partial
+// slab, whose layout is that of the other tensor-core kernels.  Roles, meeting only on mbarriers:
+//   * thread 0 issues the TMA loads of each 32-sample slice into a ring of raw stages, a 128-column block as two
+//     [32 samples x 64 columns] boxes with 128-byte swizzle: A0 (j = 2i); A0 | A1 (j = 2i + 1, B is A1);
+//     A0 | A1 | B.  The four boxes of A0 | A1 are kHfBox apart, the LBO of the N = 256 operand.  Rows past n_rows and
+//     columns past the view's width arrive as zeros;
+//   * on the tiles with j in {2i, 2i + 1} the 128 threads of the first warpgroup take the fp32 column sums of block
+//     j from the raw stages (thread m: column m), so each block's sums are written once;
+//   * the two MMA warpgroups hand a stage back once the wgmmas of the next slice are issued and those that read it
+//     have retired.
+// Per slice of a j > 2i + 1 tile that is 24 KB of TMA writes for 512 tensor clocks (two m64n256k16 per k16 step), and
+// 20 KB of wgmma operand reads per k16 step: the loads from L2, not the MMAs, are the expected bound.
+constexpr int kHfBox = kWgKC * 128;      // one [32 samples x 64 columns] 16-bit box: 4 KB
+constexpr int kHfBlock = 2 * kHfBox;     // one 128-column block
+struct HalfCfg {
+  static constexpr int kRawStage = 3 * kHfBlock;   // A0 | A1 | B
+  static constexpr int kRawStages = 8;
+  static constexpr int kBarOff = kRawStages * kRawStage;
+  static constexpr int kSmem = kBarOff + 2 * kRawStages * 8 + 1024;   // + alignment slack
+};
+static_assert(HalfCfg::kSmem <= 227 * 1024, "shared memory per block");
+static_assert(kWgKC % 16 == 0, "a slice is whole k16 steps");
+
+template <bool F16>
+__device__ __forceinline__ float half_bits_to_float(uint16_t u) {
+  if constexpr (F16)
+    return __half2float(__ushort_as_half(u));
+  else
+    return __uint_as_float((uint32_t)u << 16);
+}
+
+template <bool F16, int N>
+__device__ __forceinline__ void wgmma_half_ss(float* d, uint64_t desc_a, uint64_t desc_b) {
+  if constexpr (F16)
+    wgmma_f16_ss_mn<N>(d, desc_a, desc_b);
+  else
+    wgmma_bf16_ss_mn<N>(d, desc_a, desc_b);
+}
+
+template <bool F16>
+__global__ void __launch_bounds__(kPrThreads, 1) moments_half_pair_kernel(const __grid_constant__ WgParams p) {
+  constexpr int NR = HalfCfg::kRawStages;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // raw stages: swizzle atoms
+  uint64_t* raw_full = reinterpret_cast<uint64_t*>(smem + HalfCfg::kBarOff);
+  uint64_t* raw_empty = raw_full + NR;
+
+  int t = blockIdx.x, i = 0, rowlen = p.nblocks;   // pair tile decode
+  while (t >= rowlen) { t -= rowlen; ++i; rowlen -= 2; }
+  const int a0 = 2 * i, bj = a0 + t;
+  const int nload = min(t, 2) + 1;   // raw blocks per slice: A0 (j = 2i); A0, A1 (j = 2i + 1); A0, A1, B
+  const int bslot = nload - 1;       // where B sits in the raw stage
+  const bool diag = t < 2;           // B is an A block: its column sums
+  const bool wide = t > 0;           // N = 256 against A0 | A1, else N = 128 against A0
+  const int split = blockIdx.y;
+  const int64_t r0 = (int64_t)split * p.rows_per_split;
+  const int64_t r1 = min(r0 + p.rows_per_split, p.n_rows);
+  const int nch = r1 > r0 ? (int)((r1 - r0 + kWgKC - 1) / kWgKC) : 0;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NR; ++s) {
+      mbar_init(&raw_full[s], 1);
+      mbar_init(&raw_empty[s], 8 + (diag ? kPrXpose : 0));   // one lane of each MMA warp (+ the column-sum threads)
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (threadIdx.x < kPrXpose) {
+    // ---- TMA issue (thread 0) and the column sums of a diagonal tile ----
+    const int m = threadIdx.x;
+    if (!diag && m != 0) return;
+    auto issue = [&](int c) {
+      const int s = c % NR;
+      const int row = (int)(p.row_base + r0 + (int64_t)c * kWgKC);
+      uint8_t* dst = smem + s * HalfCfg::kRawStage;
+      mbar_arrive_expect_tx(&raw_full[s], nload * kHfBlock);
+      for (int b = 0; b < nload; ++b) {
+        const int blk = b < 2 ? a0 + b : bj;
+        const CUtensorMap* map = &p.map[p.blk_view[blk]];
+        tma_load_2d(dst + b * kHfBlock, map, &raw_full[s], p.blk_col0[blk], row);
+        tma_load_2d(dst + b * kHfBlock + kHfBox, map, &raw_full[s], p.blk_col0[blk] + 64, row);
+      }
+    };
+    if (m == 0)
+      for (int c = 0; c < min(NR, nch); ++c) issue(c);
+    // column m sits in box m / 64, element e of its 128-byte rows: 16-byte chunk e / 8, swizzled with the row
+    const int e = m & 63;
+    const uint32_t col_off = (uint32_t)(bslot * kHfBlock + (m >> 6) * kHfBox) + (uint32_t)(e & 7) * 2;
+    float csum = 0.f;
+    for (int c = 0; c < nch; ++c) {
+      const int s = c % NR;
+      if (diag) {
+        mbar_wait(&raw_full[s], (c / NR) & 1);
+        const uint8_t* src = smem + s * HalfCfg::kRawStage + col_off;
+#pragma unroll 8
+        for (int k = 0; k < kWgKC; ++k)   // a warp reads 64 bytes of one row: conflict-free
+          csum += half_bits_to_float<F16>(*reinterpret_cast<const uint16_t*>(src + k128_offset(k, e >> 3)));
+        mbar_arrive(&raw_empty[s]);
+      }
+      if (m == 0 && c + NR < nch) {   // refill the stage of slice c with slice c + NR once slice c is consumed
+        mbar_wait(&raw_empty[s], (c / NR) & 1);
+        issue(c + NR);
+      }
+    }
+    if (diag) p.partial_sum[(size_t)split * p.Dp + bj * kBlk + m] = csum;
+  } else {
+    // ---- MMA warpgroups ----
+    const int g = (threadIdx.x - kPrXpose) >> 7;   // columns 64g .. 64g + 63 of B
+    const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
+    float acc[128];
+#pragma unroll
+    for (int k = 0; k < 128; ++k) acc[k] = 0.f;
+    wgmma_fence_regs<128>(acc);   // keeps the zeroing out of the wgmma pipeline
+    // one loop per N, so that no branch sits between the wgmmas of a slice
+    auto mainloop = [&](auto n_tag) {
+      constexpr int N = decltype(n_tag)::value;
+      for (int c = 0; c < nch; ++c) {
+        const int s = c % NR;
+        mbar_wait(&raw_full[s], (c / NR) & 1);
+        const uint32_t st = smem_u32(smem + s * HalfCfg::kRawStage);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kWgKC / 16; ++kk)
+          wgmma_half_ss<F16, N>(acc, wgmma_desc_mn128(st + bslot * kHfBlock + g * kHfBox + kk * 2048, kHfBox),
+                                wgmma_desc_mn128(st + kk * 2048, kHfBox));
+        wgmma_commit();
+        wgmma_wait<1>();   // the wgmmas of slice c - 1 have retired: hand its stage back
+        if (c > 0 && lane == 0) mbar_arrive(&raw_empty[(c - 1) % NR]);
+      }
+    };
+    if (wide)
+      mainloop(std::integral_constant<int, 256>{});
+    else
+      mainloop(std::integral_constant<int, 128>{});
+    wgmma_wait_all();
+    wgmma_fence_regs<128>(acc);
+
+    // ---- epilogue: the transposed fragments -> partial slab of this split ----
+    // element r: M row 64g + 16 warp + lane / 4 + 8 ((r / 2) % 2) of B, N column 8 (r / 4) + 2 (lane % 4) + r % 2 of
+    // A0 | A1
+    float* P = p.partial + (size_t)split * p.Dp * p.Dp;
+    const int col = bj * kBlk + g * 64 + warp * 16 + (lane >> 2);
+    const int row0 = a0 * kBlk + 2 * (lane & 3);
+    const int nr = wide ? 128 : 64;
+#pragma unroll
+    for (int r = 0; r < 128; ++r)
+      if (r < nr) P[(size_t)(row0 + 8 * (r >> 2) + (r & 1)) * p.Dp + col + 8 * ((r >> 1) & 1)] = acc[r];
+  }
+}
+
+// =============================================================================================
+// exact SIMT kernel (fp32 / fp64; bf16 / fp16 converted on load to fp32), 64x64 tiles inside the same padded tile space
 // =============================================================================================
 struct SimtParams {
   const void* view_ptr[kMaxViews];
@@ -570,8 +731,9 @@ struct SimtParams {
   void* partial_sum;  // T [S][Dp]
 };
 
-template <typename T>
+template <typename E>
 __global__ void __launch_bounds__(256) moments_simt_kernel(const SimtParams p) {
+  using T = wide_t<E>;   // arithmetic type: 16-bit views are converted on load
   constexpr int KC = 16;
   __shared__ T As[KC][64];
   __shared__ T Bs[KC][64];
@@ -591,8 +753,8 @@ __global__ void __launch_bounds__(256) moments_simt_kernel(const SimtParams p) {
   int vA, cA, vB, cB;
   locate(bi * 64, vA, cA);
   locate(bj * 64, vB, cB);
-  const T* XA = static_cast<const T*>(p.view_ptr[vA]);
-  const T* XB = static_cast<const T*>(p.view_ptr[vB]);
+  const E* XA = static_cast<const E*>(p.view_ptr[vA]);
+  const E* XB = static_cast<const E*>(p.view_ptr[vB]);
   const int64_t ldA = p.view_ld[vA], ldB = p.view_ld[vB];
   const int dA = p.view_dim[vA], dB = p.view_dim[vB];
 
@@ -634,8 +796,8 @@ __global__ void __launch_bounds__(256) moments_simt_kernel(const SimtParams p) {
       const int kr = lr + 4 * i;
       const int64_t row = r + kr;
       const bool rv = row < r1;
-      As[kr][lc] = (rv && cA + lc < dA) ? XA[row * ldA + cA + lc] : T(0);
-      Bs[kr][lc] = (rv && cB + lc < dB) ? XB[row * ldB + cB + lc] : T(0);
+      As[kr][lc] = (rv && cA + lc < dA) ? (T)XA[row * ldA + cA + lc] : T(0);
+      Bs[kr][lc] = (rv && cB + lc < dB) ? (T)XB[row * ldB + cB + lc] : T(0);
     }
     __syncthreads();
 #pragma unroll
@@ -931,7 +1093,8 @@ size_t moments_workspace_bytes(int dtype, int precision, const ColumnLayout& L, 
     size_t el = dtype == 1 ? 8 : 4;
     return align256((size_t)P.num_splits * L.Dp * L.Dp * el) + align256((size_t)P.num_splits * L.Dp * el);
   }
-  TcPlan P = plan_tc(L, std::min(n_rows, tc_rows_cap(L, precision)), precision);   // sized for one pass
+  const int mode = dtype == 2 ? kModeBf16 : dtype == 3 ? kModeF16 : precision;   // CCAB_BF16, CCAB_F16
+  TcPlan P = plan_tc(L, std::min(n_rows, tc_rows_cap(L, mode)), mode);   // sized for one pass
   return align256(P.partial_bytes) + align256(P.sum_bytes) + 256;
 }
 
@@ -955,19 +1118,23 @@ EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// Row-major fp32 view (n_rows x d, row pitch ld floats) read in [32 rows x 32 columns] boxes with 128-byte swizzle
-// (see raw_offset); elements past column d or row n_rows read as zero, also in boxes that lie wholly past column d.
-int encode_view_map(CUtensorMap* map, const void* ptr, int64_t n_rows, int64_t d, int64_t ld) {
+// Row-major view (n_rows x d, row pitch ld elements) read in boxes of 32 rows x one 128-byte row with 128-byte
+// swizzle: 32 fp32 columns (see raw_offset), or 64 bf16 / fp16 columns (half = 1, 2).  Elements past column d or row
+// n_rows read as zero, also in boxes that lie wholly past column d.
+int encode_view_map(CUtensorMap* map, const void* ptr, int64_t n_rows, int64_t d, int64_t ld, int half = 0) {
   EncodeTiledFn enc = encode_fn();
   if (!enc) {
     set_error("cuTensorMapEncodeTiled entry point not available (driver too old?)");
     return -2;
   }
   cuuint64_t gdim[2] = {(cuuint64_t)d, (cuuint64_t)n_rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)ld * 4};
-  cuuint32_t box[2] = {32, (cuuint32_t)kWgKC};
+  cuuint64_t gstride[1] = {(cuuint64_t)ld * (half ? 2 : 4)};
+  cuuint32_t box[2] = {half ? 64u : 32u, (cuuint32_t)kWgKC};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
+  const CUtensorMapDataType type = half == 1   ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                   : half == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                               : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  CUresult r = enc(map, type, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -990,10 +1157,17 @@ int moments_tf32_pass(const ColumnLayout& L, WgParams& prm, int64_t row_base, in
 int moments_tf32(const ColumnLayout& L, const void* const* views, const int64_t* lds, int64_t n_rows, int mode,
                  double* moments_out, void* ws, size_t ws_bytes, cudaStream_t stream) {
   CCAB_CHECK_ARG(n_rows >= 1 && n_rows < (int64_t)1 << 31, "n_rows out of range");
-  for (int v = 0; v < L.n_views; ++v)
-    CCAB_CHECK_ARG((reinterpret_cast<uintptr_t>(views[v]) & 15) == 0 && lds[v] % 4 == 0,
-                   "TF32 moments need 16-byte aligned views and lds %% 4 == 0 (view %d: ld %lld)", v,
-                   (long long)lds[v]);
+  const int half = mode == kModeBf16 ? 1 : mode == kModeF16 ? 2 : 0;
+  for (int v = 0; v < L.n_views; ++v) {
+    if (half)
+      CCAB_CHECK_ARG((reinterpret_cast<uintptr_t>(views[v]) & 15) == 0 && lds[v] % 8 == 0,
+                     "16-bit tensor-core moments need 16-byte aligned views and lds %% 8 == 0 (view %d: ld %lld)", v,
+                     (long long)lds[v]);
+    else
+      CCAB_CHECK_ARG((reinterpret_cast<uintptr_t>(views[v]) & 15) == 0 && lds[v] % 4 == 0,
+                     "TF32 moments need 16-byte aligned views and lds %% 4 == 0 (view %d: ld %lld)", v,
+                     (long long)lds[v]);
+  }
   {
     int dev = 0;   // bind the primary context to this thread before the driver-API tensor-map encoder
     CCAB_CUDA(cudaGetDevice(&dev));
@@ -1002,7 +1176,7 @@ int moments_tf32(const ColumnLayout& L, const void* const* views, const int64_t*
   WgParams prm;
   memset(&prm, 0, sizeof(prm));
   for (int v = 0; v < L.n_views; ++v) {
-    int rc = encode_view_map(&prm.map[v], views[v], n_rows, L.dims[v], lds[v]);
+    int rc = encode_view_map(&prm.map[v], views[v], n_rows, L.dims[v], lds[v], half);
     if (rc) return rc;
   }
   int b = 0;
@@ -1034,6 +1208,15 @@ int launch_wgmma(dim3 grid, const WgParams& prm, cudaStream_t stream) {
   return 0;
 }
 
+template <bool F16>
+int launch_half_pair(int num_splits, const WgParams& prm, cudaStream_t stream) {
+  CCAB_CUDA(cudaFuncSetAttribute(moments_half_pair_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 HalfCfg::kSmem));
+  moments_half_pair_kernel<F16>
+      <<<dim3(pair_tiles(prm.nblocks), num_splits), kPrThreads, HalfCfg::kSmem, stream>>>(prm);
+  return 0;
+}
+
 int launch_x3b_pair(int num_splits, const WgParams& prm, cudaStream_t stream) {
   CCAB_CUDA(cudaFuncSetAttribute(moments_x3b_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  PairCfg::kSmem));
@@ -1061,9 +1244,11 @@ int moments_tf32_pass(const ColumnLayout& L, WgParams& prm, int64_t row_base, in
   prm.Dp = L.Dp;
   dim3 grid(P.ntiles, P.num_splits);
   if (g_prof_on) cudaEventRecord(g_prof_e0, stream);
-  int rc = mode == 3   ? launch_x3b_pair(P.num_splits, prm, stream)
-           : mode != 0 ? launch_wgmma<K1Mode::X3>(grid, prm, stream)
-                       : launch_wgmma<K1Mode::TF32>(grid, prm, stream);
+  int rc = mode == kModeBf16 ? launch_half_pair<false>(P.num_splits, prm, stream)
+           : mode == kModeF16  ? launch_half_pair<true>(P.num_splits, prm, stream)
+           : mode == 3         ? launch_x3b_pair(P.num_splits, prm, stream)
+           : mode != 0         ? launch_wgmma<K1Mode::X3>(grid, prm, stream)
+                               : launch_wgmma<K1Mode::TF32>(grid, prm, stream);
   if (rc) return rc;
   count_launches(1);
   CCAB_CUDA(cudaGetLastError());
@@ -1081,9 +1266,10 @@ int moments_tf32_pass(const ColumnLayout& L, WgParams& prm, int64_t row_base, in
 }
 }  // namespace
 
-template <typename T>
+template <typename E>
 int moments_simt(const ColumnLayout& L, const void* const* views, const int64_t* lds, int64_t n_rows,
                  double* moments_out, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  using T = wide_t<E>;   // partials of 16-bit views are fp32
   CCAB_CHECK_ARG(n_rows >= 1, "n_rows must be positive");
   SimtPlan P = plan_simt(L, n_rows);
   const size_t pb = align256((size_t)P.num_splits * L.Dp * L.Dp * sizeof(T));
@@ -1108,10 +1294,10 @@ int moments_simt(const ColumnLayout& L, const void* const* views, const int64_t*
   // partial sums of non-diagonal 64-blocks inside a 128-block are never written by the kernel: the
   // reducer only reads what a tile wrote (block-triangle test at 64 granularity).
   dim3 grid(P.ntiles, P.num_splits);
-  if constexpr (std::is_same<T, double>::value)
+  if constexpr (std::is_same<E, double>::value)
     moments_dmma_kernel<<<grid, 256, 0, stream>>>(prm);
   else
-    moments_simt_kernel<T><<<grid, 256, 0, stream>>>(prm);
+    moments_simt_kernel<E><<<grid, 256, 0, stream>>>(prm);
   count_launches(1);
   CCAB_CUDA(cudaGetLastError());
   const size_t total = (size_t)L.Dp * L.Dp + L.Dp;
@@ -1126,6 +1312,10 @@ int moments_simt(const ColumnLayout& L, const void* const* views, const int64_t*
 template int moments_simt<float>(const ColumnLayout&, const void* const*, const int64_t*, int64_t, double*, void*,
                                  size_t, cudaStream_t);
 template int moments_simt<double>(const ColumnLayout&, const void* const*, const int64_t*, int64_t, double*, void*,
+                                  size_t, cudaStream_t);
+template int moments_simt<__nv_bfloat16>(const ColumnLayout&, const void* const*, const int64_t*, int64_t, double*,
+                                         void*, size_t, cudaStream_t);
+template int moments_simt<__half>(const ColumnLayout&, const void* const*, const int64_t*, int64_t, double*, void*,
                                   size_t, cudaStream_t);
 
 // =============================================================================================
@@ -1322,16 +1512,19 @@ int moments_exchange_nvls(const ColumnLayout& L, double* mom, double n_local, do
 // unshift_kernel: the float64 correction above on the padded moment buffer (upper block triangle)
 // =============================================================================================
 template <typename T>
-__global__ void pilot_kernel(const T* __restrict__ X, int64_t rows, int d, int64_t ld, T* __restrict__ x0,
+__device__ __forceinline__ double as_f64(T v) { return (double)(wide_t<T>)v; }
+
+template <typename T>
+__global__ void pilot_kernel(const T* __restrict__ X, int64_t rows, int d, int64_t ld, wide_t<T>* __restrict__ x0,
                              float* __restrict__ ratio_max) {
   __shared__ double s1[32][33], s2[32][33];
   const int j = blockIdx.x * 32 + (threadIdx.x & 31);
   const int rg = threadIdx.x >> 5;
   double a = 0.0, b = 0.0;
-  const double ref = j < d ? (double)X[j] : 0.0;     // first row as a provisional origin: the pilot itself must not cancel
+  const double ref = j < d ? as_f64(X[j]) : 0.0;     // first row as a provisional origin: the pilot itself must not cancel
   if (j < d)
     for (int64_t i = rg; i < rows; i += 32) {
-      const double v = (double)X[i * ld + j] - ref;
+      const double v = as_f64(X[i * ld + j]) - ref;
       a += v;
       b += v * v;
     }
@@ -1344,20 +1537,20 @@ __global__ void pilot_kernel(const T* __restrict__ X, int64_t rows, int d, int64
     const double mean = sa / (double)rows;
     const double var = fmax(sb / (double)rows - mean * mean, 0.0);
     const double m0 = ref + mean;
-    x0[j] = (T)m0;
+    x0[j] = (wide_t<T>)m0;
     const double r = var > 0.0 ? m0 * m0 / var : (m0 != 0.0 ? 1e30 : 0.0);
     atomicMax(reinterpret_cast<unsigned*>(ratio_max), __float_as_uint((float)fmin(r, 1e30)));
   }
 }
 
 template <typename T>
-__global__ void shift_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const T* __restrict__ x0,
-                             T* __restrict__ Xs, int64_t lds) {
+__global__ void shift_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const wide_t<T>* __restrict__ x0,
+                             wide_t<T>* __restrict__ Xs, int64_t lds) {
   const int64_t total = n * (int64_t)d;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = i / d;
     const int c = (int)(i - r * d);
-    Xs[r * lds + c] = X[r * ldx + c] - x0[c];
+    Xs[r * lds + c] = (wide_t<T>)X[r * ldx + c] - x0[c];
   }
 }
 
@@ -1394,7 +1587,7 @@ __global__ void unshift_sums_kernel(const UnshiftParams p, double* __restrict__ 
 }
 
 template <typename T>
-int column_pilot(const T* X, int64_t rows, int d, int64_t ld, T* x0, float* ratio_max, cudaStream_t stream) {
+int column_pilot(const T* X, int64_t rows, int d, int64_t ld, wide_t<T>* x0, float* ratio_max, cudaStream_t stream) {
   CCAB_CHECK_ARG(rows >= 1 && d >= 1 && ld >= d, "bad pilot shape");
   pilot_kernel<T><<<(unsigned)ceil_div(d, 32), 1024, 0, stream>>>(X, rows, d, ld, x0, ratio_max);
   count_launches(1);
@@ -1402,7 +1595,8 @@ int column_pilot(const T* X, int64_t rows, int d, int64_t ld, T* x0, float* rati
   return 0;
 }
 template <typename T>
-int shift_rows(const T* X, int64_t n, int d, int64_t ldx, const T* x0, T* Xs, int64_t lds, cudaStream_t stream) {
+int shift_rows(const T* X, int64_t n, int d, int64_t ldx, const wide_t<T>* x0, wide_t<T>* Xs, int64_t lds,
+               cudaStream_t stream) {
   const int64_t total = n * (int64_t)d;
   if (total == 0) return 0;
   shift_kernel<T><<<(unsigned)std::min<int64_t>(ceil_div(total, 256), (int64_t)sm_count() * 16), 256, 0, stream>>>(
@@ -1415,6 +1609,11 @@ template int column_pilot<float>(const float*, int64_t, int, int64_t, float*, fl
 template int column_pilot<double>(const double*, int64_t, int, int64_t, double*, float*, cudaStream_t);
 template int shift_rows<float>(const float*, int64_t, int, int64_t, const float*, float*, int64_t, cudaStream_t);
 template int shift_rows<double>(const double*, int64_t, int, int64_t, const double*, double*, int64_t, cudaStream_t);
+template int column_pilot<__nv_bfloat16>(const __nv_bfloat16*, int64_t, int, int64_t, float*, float*, cudaStream_t);
+template int column_pilot<__half>(const __half*, int64_t, int, int64_t, float*, float*, cudaStream_t);
+template int shift_rows<__nv_bfloat16>(const __nv_bfloat16*, int64_t, int, int64_t, const float*, float*, int64_t,
+                                       cudaStream_t);
+template int shift_rows<__half>(const __half*, int64_t, int, int64_t, const float*, float*, int64_t, cudaStream_t);
 
 int moments_unshift(const ColumnLayout& L, double* mom, const void* const* x0, int is_f64, double n,
                     cudaStream_t stream) {

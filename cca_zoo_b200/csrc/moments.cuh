@@ -1,5 +1,8 @@
 // Block-moment stage (kernels K1/K2 of DESIGN.md): M = [X1..Xm]^T [X1..Xm], s = 1^T X.
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 
 namespace ccab {
@@ -23,14 +26,32 @@ struct ColumnLayout {
 
 int make_layout(int n_views, const int64_t* dims, ColumnLayout* out);
 
+// Arithmetic type of a view element: 16-bit views are converted on load and accumulated in fp32, and their pilot
+// origin and shifted copy are fp32.
+template <typename T>
+struct Wide { using type = T; };
+template <>
+struct Wide<__nv_bfloat16> { using type = float; };
+template <>
+struct Wide<__half> { using type = float; };
+template <typename T>
+using wide_t = typename Wide<T>::type;
+
 // --- launchers (all asynchronous on `stream`) -------------------------------------------------
 // precision: 0 = TF32 single pass (wgmma), 1 = 3xTF32 split (wgmma), 2 = exact SIMT FMA,
 //            3 = 3xTF32 with the two cross terms as bf16 MMAs (hi*hi in TF32): 2 instead of 3 units of tensor work,
 //            the same split plan and passes as 1.
+// dtype: CCAB_F32, CCAB_F64, CCAB_BF16 or CCAB_F16; every tensor precision of a 16-bit dtype is the 16-bit wgmma
+// kernel (mode kModeBf16 / kModeF16 of moments_tf32).
 size_t moments_workspace_bytes(int dtype, int precision, const ColumnLayout& L, int64_t n_rows);
 
+// modes of moments_tf32 beyond the float32 precisions 0, 1 and 3: bf16 / fp16 views, one wgmma per k16 step (the
+// products are exact in fp32), with the split plan and passes of the 3xTF32 modes
+constexpr int kModeBf16 = 4, kModeF16 = 5;
+
 int moments_tf32(const ColumnLayout& L, const void* const* views, const int64_t* lds, int64_t n_rows,
-                 int mode /* 0, 1 or 3 */, double* moments_out, void* ws, size_t ws_bytes, cudaStream_t stream);
+                 int mode /* 0, 1, 3, kModeBf16 or kModeF16 */, double* moments_out, void* ws, size_t ws_bytes,
+                 cudaStream_t stream);
 
 template <typename T>
 int moments_simt(const ColumnLayout& L, const void* const* views, const int64_t* lds, int64_t n_rows,
@@ -52,10 +73,12 @@ int moments_unpack(const ColumnLayout& L, const double* packed, double* moments,
 
 // Shifted accumulation: pilot statistics of the leading rows, Xs = X - x0, and the float64 correction that turns the
 // moments of the shifted data back into raw moments (see moments.cu).
+// x0 and Xs are wide_t<T>: float32 for 16-bit views.
 template <typename T>
-int column_pilot(const T* X, int64_t rows, int d, int64_t ld, T* x0, float* ratio_max, cudaStream_t stream);
+int column_pilot(const T* X, int64_t rows, int d, int64_t ld, wide_t<T>* x0, float* ratio_max, cudaStream_t stream);
 template <typename T>
-int shift_rows(const T* X, int64_t n, int d, int64_t ldx, const T* x0, T* Xs, int64_t lds, cudaStream_t stream);
+int shift_rows(const T* X, int64_t n, int d, int64_t ldx, const wide_t<T>* x0, wide_t<T>* Xs, int64_t lds,
+               cudaStream_t stream);
 int moments_unshift(const ColumnLayout& L, double* moments, const void* const* x0, int is_f64, double n,
                     cudaStream_t stream);
 

@@ -23,6 +23,12 @@ loss stage runs on the global moments with the global count N read on the device
 backward is the exact derivative of that loss with respect to its own rows, centred by the saved global means, with no
 collective (``ccab_ccaloss_bwd_global``, ``ccab_row_sub_scale``).  Every route decision is taken from exchanged data, so
 all ranks take the same route and raise at the same call.
+
+bfloat16 / float16 representations (an encoder under ``torch.autocast``; CCALoss / MCCALoss / GCCALoss) take the
+global-batch route also in a single process, where nothing is exchanged and N is a device scalar holding n: the moment
+pass reads the 16-bit representations as they are (16-bit wgmma, or fp32 FMA for narrow batches), the loss stage runs
+in float32, and the backward runs the float32 global backward on float32 copies of the saved representations made
+inside ``backward``; the gradients come back in the representation's dtype.
 """
 from __future__ import annotations
 
@@ -30,6 +36,7 @@ import torch
 import torch.nn as nn
 
 from .. import ops, parallel
+from ..ops import HALF_DTYPES
 
 
 def _require_cuda(name, *tensors):
@@ -49,7 +56,8 @@ def _resolve_precision(precision, zs):
         return "exact"
     if precision == "auto":
         precision = "tf32x3b" if sum(z.shape[1] for z in zs) > 256 else "exact"
-    if precision != "exact" and not all(z.data_ptr() % 16 == 0 and z.stride(0) % 4 == 0 for z in zs):
+    if precision != "exact" and not all(z.data_ptr() % 16 == 0 and (z.stride(0) * z.element_size()) % 16 == 0
+                                        for z in zs):
         return "exact"
     return precision
 
@@ -139,17 +147,30 @@ def _is_global(global_batch, group):
     return bool(global_batch) and parallel.is_distributed(group)
 
 
-def _exchange(zd, precision, group):
+def _exchange(zd, precision, group, exchange=True):
     """The ONE collective of a global-batch forward: this rank's moment buffer summed over the ranks.  Returns
-    (moments of the global batch, N as a 1-element float64 device tensor) -- nothing is read back."""
+    (moments of the global batch, N as a 1-element float64 device tensor) -- nothing is read back.  ``exchange=False``
+    (16-bit representations in a single process): the local moments, and n as that device scalar."""
     dims = [int(z.shape[1]) for z in zd]
     n_local = int(zd[0].shape[0])
     if n_local > 0:
         mom = ops.moments(zd, precision=precision)
     else:   # no rows here: contribute zeros (raising would leave the other ranks waiting in the exchange)
         mom = torch.zeros(ops.moments_size(dims), dtype=torch.float64, device=zd[0].device)
+    if not exchange:
+        return mom, torch.full((1,), float(n_local), dtype=torch.float64, device=mom.device)
     mom, _, n_dev = parallel.allreduce_moments_lazy(mom, n_local, group, dims)
     return mom, n_dev
+
+
+def _compute_dtype(dt):
+    """dtype of the loss stage and the backward: float32 for 16-bit representations."""
+    return torch.float32 if dt in HALF_DTYPES else dt
+
+
+def _widen(zs):
+    """float32 copies of saved 16-bit representations (made inside ``backward``), the others as they are."""
+    return [z.float() if z.dtype in HALF_DTYPES else z for z in zs]
 
 
 def _global_count(n_dev, what):
@@ -174,10 +195,13 @@ def _eigen_route_global(mom, n_dev, d1, d2, eps, dtype):
     return loss, torch.cat([saved, n_dev.to(dtype).reshape(1)])
 
 
+_LOSS_DTYPES = (torch.float32, torch.float64, torch.bfloat16, torch.float16)
+
+
 def _check_pair(z1, z2, name):
     _require_cuda(name, z1, z2)
-    if z1.dtype != z2.dtype or z1.dtype not in (torch.float32, torch.float64):
-        raise ValueError("representations must share a float32/float64 dtype")
+    if z1.dtype != z2.dtype or z1.dtype not in _LOSS_DTYPES:
+        raise ValueError("representations must share a float32/float64/bfloat16/float16 dtype")
 
 
 class _CCALossFn(torch.autograd.Function):
@@ -213,20 +237,22 @@ class _CCALossFn(torch.autograd.Function):
 
 
 class _CCALossGlobalFn(torch.autograd.Function):
-    """CCALoss of the global batch: this rank's rows, the moments of all ranks (see the module docstring)."""
+    """CCALoss of the global batch: this rank's rows, the moments of all ranks (see the module docstring).  With
+    ``glob=False`` (16-bit representations in a single process) the same body without the exchange."""
 
     @staticmethod
-    def forward(ctx, z1, z2, eps, precision, status, sync, group):
+    def forward(ctx, z1, z2, eps, precision, status, sync, group, glob=True):
         _check_pair(z1, z2, "CCALoss")
         n, d1, d2 = int(z1.shape[0]), int(z1.shape[1]), int(z2.shape[1])
+        dt = _compute_dtype(z1.dtype)
         z1d, z2d = _row_major(z1), _row_major(z2)
-        mom, n_dev = _exchange([z1d, z2d], _resolve_precision(precision, [z1d, z2d]), group)
+        mom, n_dev = _exchange([z1d, z2d], _resolve_precision(precision, [z1d, z2d]), group, glob)
         width = max(d1, d2)
         # n - 1 >= width here implies N - 1 >= width: no read-back.  Only a narrower shard reads N, and N (exchanged)
         # decides for every rank alike.
         eigen = n - 1 < width and _global_count(n_dev, "CCALoss") - 1 < width
         if not eigen:
-            loss, saved, flags = ops.ccaloss_fwd_moments(mom, n_dev, d1, d2, eps, z1.dtype)
+            loss, saved, flags = ops.ccaloss_fwd_moments(mom, n_dev, d1, d2, eps, dt)
             if sync:
                 f = flags.tolist()                            # flags of the global moments: the same on every rank
                 if f[2]:
@@ -235,16 +261,17 @@ class _CCALossGlobalFn(torch.autograd.Function):
             else:
                 status.push(flags)
         if eigen:
-            loss, saved = _eigen_route_global(mom, n_dev, d1, d2, eps, z1.dtype)
+            loss, saved = _eigen_route_global(mom, n_dev, d1, d2, eps, dt)
         ctx.save_for_backward(z1d, z2d, saved)
         return loss.reshape(()).clone()
 
     @staticmethod
     def backward(ctx, grad_out):
         z1, z2, saved = ctx.saved_tensors
-        go = grad_out.to(z1.dtype).reshape(1).contiguous()
-        g1, g2 = ops.ccaloss_bwd_global(z1, z2, saved, go)
-        return g1, g2, None, None, None, None, None
+        z1w, z2w = _widen([z1, z2])
+        go = grad_out.to(z1w.dtype).reshape(1).contiguous()
+        g1, g2 = ops.ccaloss_bwd_global(z1w, z2w, saved, go)
+        return g1.to(z1.dtype), g2.to(z2.dtype), None, None, None, None, None, None
 
 
 class CCALoss(nn.Module):
@@ -267,6 +294,10 @@ class CCALoss(nn.Module):
             per-replica statistics).
         process_group: the ranks whose batches form the global batch (``None``: the default group, as in
             ``torch.nn.SyncBatchNorm``).
+
+    Representations may be float32, float64, bfloat16 or float16 (both of one dtype).  16-bit representations are
+    read by the moment pass as they are; the loss (float32) and the float32 backward follow the global-batch route
+    (see the module docstring), and the gradients have the representations' dtype.
     """
 
     def __init__(self, eps: float = 1e-5, precision: str = "auto", verify: str = "lazy", global_batch: bool = False,
@@ -293,9 +324,10 @@ class CCALoss(nn.Module):
             )
         self._status.poll()
         z1, z2 = representations
-        if _is_global(self.global_batch, self.process_group):
+        glob = _is_global(self.global_batch, self.process_group)
+        if glob or z1.dtype in HALF_DTYPES:
             return _CCALossGlobalFn.apply(z1, z2, float(self.eps), self.precision, self._status, self.verify == "sync",
-                                          self.process_group)
+                                          self.process_group, glob)
         return _CCALossFn.apply(z1, z2, float(self.eps), self.precision, self._status, self.verify == "sync")
 
 
@@ -428,21 +460,22 @@ class _MCCALossFn(torch.autograd.Function):
 
 
 class _MCCALossGlobalFn(torch.autograd.Function):
-    """MCCALoss of the global batch: one exchange, the pairs from the global C; backward with the global means."""
+    """MCCALoss of the global batch: one exchange, the pairs from the global C; backward with the global means.  With
+    ``glob=False`` (16-bit representations in a single process) the same body without the exchange."""
 
     @staticmethod
-    def forward(ctx, eps, precision, status, sync, group, *zs):
+    def forward(ctx, eps, precision, status, sync, group, glob, *zs):
         _require_cuda("MCCALoss", *zs)
-        dt = zs[0].dtype
-        if dt not in (torch.float32, torch.float64) or any(z.dtype != dt for z in zs):
-            raise ValueError("representations must share a float32/float64 dtype")
+        if zs[0].dtype not in _LOSS_DTYPES or any(z.dtype != zs[0].dtype for z in zs):
+            raise ValueError("representations must share a float32/float64/bfloat16/float16 dtype")
+        dt = _compute_dtype(zs[0].dtype)
         n, m = int(zs[0].shape[0]), len(zs)
         zd = [_row_major(z) for z in zs]
         dims = [int(z.shape[1]) for z in zd]
         off = [0]
         for d in dims:
             off.append(off[-1] + d)
-        mom, n_dev = _exchange(zd, _resolve_precision(precision, zd), group)
+        mom, n_dev = _exchange(zd, _resolve_precision(precision, zd), group, glob)
         C, mean = ops.covariance(mom, dims, n_dev, center=True, dtype=dt)
         eigen = n - 1 < max(dims) and _global_count(n_dev, "MCCALoss") - 1 < max(dims)
         W = None                                   # whitening rows, on the eigen route only
@@ -470,7 +503,8 @@ class _MCCALossGlobalFn(torch.autograd.Function):
     def backward(ctx, grad_out):
         m = ctx.m
         mean, n_dev, *t = ctx.saved_tensors
-        zs, G = t[:m], t[m:2 * m]
+        in_dt = [z.dtype for z in t[:m]]
+        zs, G = _widen(t[:m]), t[m:2 * m]
         P = dict(zip(ctx.pairs, t[2 * m:]))
         dt = zs[0].dtype
         # dL/dz_i = 2/(N-1) (z_i G_i - sum_j z_j P_ji - 1 r_i^T) go, r_i the same product of the global mean rows
@@ -480,12 +514,12 @@ class _MCCALossGlobalFn(torch.autograd.Function):
             mus.append(mean[o:o + z.shape[1]].reshape(1, -1))
             o += z.shape[1]
         if zs[0].shape[0] == 0:
-            return (None, None, None, None, None, *[torch.zeros_like(z) for z in zs])
+            return (None, None, None, None, None, None, *[torch.zeros_like(z, dtype=d) for z, d in zip(zs, in_dt)])
         rows = _mcca_products(mus, G, P, 1.0)
         grads = _mcca_products(list(zs), G, P, 1.0)
         for g, r in zip(grads, rows):
             ops.row_sub_scale_(g, r.reshape(-1), s)
-        return (None, None, None, None, None, *grads)
+        return (None, None, None, None, None, None, *[g.to(d) for g, d in zip(grads, in_dt)])
 
 
 class MCCALoss(nn.Module):
@@ -496,7 +530,9 @@ class MCCALoss(nn.Module):
 
     ``global_batch`` / ``process_group`` as in ``CCALoss`` (2 to 8 views): one exchange per forward, and all pairs come
     from the global block covariance.  There ``verify="sync"`` reads the replicated status and, if some S_ii failed,
-    evaluates every pair through the eigen route from the same global covariance (no per-pair exchanges)."""
+    evaluates every pair through the eigen route from the same global covariance (no per-pair exchanges).
+    bfloat16 / float16 representations (2 to 8, one dtype) take that route in a single process too, without the
+    exchange (see the module docstring)."""
 
     def __init__(self, eps: float = 1e-5, precision: str = "auto", verify: str = "lazy", global_batch: bool = False,
                  process_group=None) -> None:
@@ -518,12 +554,14 @@ class MCCALoss(nn.Module):
 
     def forward(self, representations: list[torch.Tensor]) -> torch.Tensor:
         n_views = len(representations)
-        if _is_global(self.global_batch, self.process_group):
+        glob = _is_global(self.global_batch, self.process_group)
+        if glob or (n_views and representations[0].dtype in HALF_DTYPES):
             if not 2 <= n_views <= 8:
-                raise ValueError(f"MCCALoss with global_batch=True takes 2 to 8 representations, got {n_views}.")
+                what = "with global_batch=True" if glob else "with 16-bit representations"
+                raise ValueError(f"MCCALoss {what} takes 2 to 8 representations, got {n_views}.")
             self._global_status.poll()
             return _MCCALossGlobalFn.apply(float(self.eps), self.precision, self._global_status, self.verify == "sync",
-                                           self.process_group, *representations)
+                                           self.process_group, glob, *representations)
         n = representations[0].shape[0]
         lazy_ok = (self.verify == "lazy" and 2 <= n_views <= 8
                    and n - 1 >= max(int(z.shape[1]) for z in representations))
@@ -552,17 +590,19 @@ class _GCCALossFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, eps, precision, glob, group, *zs):
         _require_cuda("GCCALoss", *zs)
-        dt = zs[0].dtype
-        if dt not in (torch.float32, torch.float64) or any(z.dtype != dt for z in zs):
-            raise ValueError("representations must share a float32/float64 dtype")
+        if zs[0].dtype not in _LOSS_DTYPES or any(z.dtype != zs[0].dtype for z in zs):
+            raise ValueError("representations must share a float32/float64/bfloat16/float16 dtype")
+        dt = _compute_dtype(zs[0].dtype)
+        # 16-bit representations take the global-batch body in a single process too, without the exchange
+        route_global = glob or zs[0].dtype in HALF_DTYPES
         n = zs[0].shape[0]
         dims = [int(z.shape[1]) for z in zs]
         D, k = sum(dims), dims[0]
         zd = [z.detach() for z in zs]
         mean = None
-        if glob:
+        if route_global:
             # global batch: one exchange; N is read back (the Jacobi sweeps below read back anyway) and replaces n
-            mom, n_dev = _exchange(zd, precision, group)
+            mom, n_dev = _exchange(zd, precision, group, glob)
             C, mean = ops.covariance(mom, dims, n_dev, center=True, dtype=dt)
             n = _global_count(n_dev, "GCCALoss")
             _check_finite(C, "GCCALoss")
@@ -580,7 +620,7 @@ class _GCCALossFn(torch.autograd.Function):
         K = 0.5 * (K + K.T)
         evals, Ut = ops.syevj(K)                              # descending; rows of Ut are eigenvectors
         lam_k = evals[:k].contiguous()
-        ctx.n, ctx.dims, ctx.glob = n, dims, glob
+        ctx.n, ctx.dims, ctx.glob = n, dims, route_global
         ctx.save_for_backward(C, Wt, lam_k, Ut[:k].contiguous(), mean, *zd)
         return -lam_k.sum()
 
@@ -595,7 +635,8 @@ class _GCCALossFn(torch.autograd.Function):
         A = ops.gemm(C, Q, alpha=float(n - 1))                            # D x k
         B = ops.gemm(Wt, ops.gemm(Wt, A), transa=True)                    # blkdiag(S_i^-1) A
         if ctx.glob:
-            return (None, None, None, None, *_gcca_global_grads(zs, dims, Q, B, mean, n, grad_out))
+            grads = _gcca_global_grads(_widen(zs), dims, Q, B, mean, n, grad_out)
+            return (None, None, None, None, *[g.to(z.dtype) for g, z in zip(grads, zs)])
         Y = torch.zeros((n, k), dtype=C.dtype, device=C.device)
         off = 0
         for z, d in zip(zs, dims):
@@ -653,7 +694,9 @@ class GCCALoss(nn.Module):
     Same constructor and ``forward(list[Tensor]) -> 0-dim Tensor`` as the reference, so it plugs into
     ``DCCA(objective=...)`` and is what ``DGCCA`` uses (cca_zoo/deep/_dgcca.py:70).  At most 8 views.
     ``global_batch`` / ``process_group`` as in ``CCALoss``: one exchange per forward, and the eigenproblem of the
-    global block covariance (its Jacobi sweeps read back, as the per-replica route's do, and so does N)."""
+    global block covariance (its Jacobi sweeps read back, as the per-replica route's do, and so does N).
+    bfloat16 / float16 representations take that route in a single process too, without the exchange (see the module
+    docstring)."""
 
     def __init__(self, eps: float = 1e-5, precision: str = "exact", global_batch: bool = False,
                  process_group=None) -> None:

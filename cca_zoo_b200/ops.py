@@ -11,7 +11,9 @@ import torch
 
 from . import _lib
 
-_DT = {torch.float32: _lib.F32, torch.float64: _lib.F64}
+_DT = {torch.float32: _lib.F32, torch.float64: _lib.F64, torch.bfloat16: _lib.BF16, torch.float16: _lib.F16}
+#: 16-bit view dtypes: accepted by the moment pass (and its shifted accumulation) only
+HALF_DTYPES = (torch.bfloat16, torch.float16)
 
 
 def _require_cuda(t: torch.Tensor, name: str) -> None:
@@ -59,6 +61,8 @@ def moments(views, precision: str = "tf32x3b") -> torch.Tensor:
 
     Returns the additive double buffer ``[Dp*Dp + Dp]`` (see ccab_moments in include/ccab200.h).
     precision: "tf32" | "tf32x3" | "tf32x3b" (3xTF32 with bf16 cross terms) | "exact" (float64 views always use "exact").
+    bfloat16 / float16 views: every tensor precision is the 16-bit wgmma kernel (exact products, fp32 runs of at most
+    2048 samples summed in float64); "exact" is fp32 FMA on CUDA cores.
     """
     lib = _lib.load()
     if not (1 <= len(views) <= _lib.MAX_VIEWS):
@@ -67,7 +71,7 @@ def moments(views, precision: str = "tf32x3b") -> torch.Tensor:
     for v in views:
         _require_cuda(v, "view")
         if v.dtype != dt or v.dtype not in _DT:
-            raise ValueError("views must share one dtype (float32 or float64)")
+            raise ValueError("views must share one dtype (float32, float64, bfloat16 or float16)")
         if v.shape[0] != views[0].shape[0]:
             raise ValueError("All views must have the same number of samples.")
         if v.device != views[0].device:
@@ -139,21 +143,23 @@ def moments_exchange_nvls(mom: torch.Tensor, dims, n_local, sym: torch.Tensor, m
 
 
 #: a column whose pilot mean^2 / variance exceeds this is accumulated shifted (relative covariance error of the float32
-#: moment kernels ~ 1e-6 * ratio; float64 kernels have 9 more digits and never need it below 1e8)
-SHIFT_RATIO = {torch.float32: 16.0, torch.float64: 1e8}
+#: moment kernels ~ 1e-6 * ratio; float64 kernels have 9 more digits and never need it below 1e8; 16-bit views are
+#: accumulated in the same class of fp32 runs as float32)
+SHIFT_RATIO = {torch.float32: 16.0, torch.float64: 1e8, torch.bfloat16: 16.0, torch.float16: 16.0}
 PILOT_ROWS = 4096
 
 
 def column_pilot(views):
     """Per view x0 (pilot column means of the leading rows, device tensors in the views' dtype) and the largest
-    mean^2 / variance over all columns (ONE host read-back: it decides whether an extra pass is worth taking)."""
+    mean^2 / variance over all columns (ONE host read-back: it decides whether an extra pass is worth taking).
+    x0 of a 16-bit view is float32."""
     lib = _lib.load()
     ratio = torch.zeros(1, dtype=torch.float32, device=views[0].device)
     x0 = []
     for v in views:
         _require_cuda(v, "view")
         vv = v if v.stride(1) == 1 else v.contiguous()
-        o = torch.empty(v.shape[1], dtype=v.dtype, device=v.device)
+        o = torch.empty(v.shape[1], dtype=torch.float32 if v.dtype in HALF_DTYPES else v.dtype, device=v.device)
         with torch.cuda.device(v.device):
             rc = lib.ccab_column_pilot(_DT[v.dtype], _ptr(vv), min(int(v.shape[0]), PILOT_ROWS), int(v.shape[1]),
                                        vv.stride(0), _ptr(o), _ptr(ratio), _stream(v))
@@ -163,12 +169,14 @@ def column_pilot(views):
 
 
 def shift_rows(v, x0):
-    """v - x0 (row-major copy with a TMA-friendly leading dimension)."""
+    """v - x0 (row-major copy with a TMA-friendly leading dimension; float32 for a 16-bit view, whose float32 x0 it
+    subtracts, so that the shifted copy is not rounded back to 16 bits)."""
     lib = _lib.load()
     vv = v if v.stride(1) == 1 else v.contiguous()
-    per = 16 // v.element_size()
+    out_dt = torch.float32 if v.dtype in HALF_DTYPES else v.dtype
+    per = 16 // out_dt.itemsize
     ld = (v.shape[1] + per - 1) // per * per
-    out = torch.empty((v.shape[0], ld), dtype=v.dtype, device=v.device)
+    out = torch.empty((v.shape[0], ld), dtype=out_dt, device=v.device)
     with torch.cuda.device(v.device):
         rc = lib.ccab_shift_rows(_DT[v.dtype], _ptr(vv), int(v.shape[0]), int(v.shape[1]), vv.stride(0), _ptr(x0),
                                  _ptr(out), ld, _stream(v))
@@ -192,6 +200,7 @@ def moments_safe(views, precision: str = "tf32x3b", x0=None):
     """``moments`` with the shifted accumulation when it matters: a pilot over the leading rows decides (one tiny
     kernel per view and one scalar read-back); badly centred views are accumulated as X - x0 and the raw moments are
     rebuilt in float64.  ``x0`` given = shift by it unconditionally (streamed fits keep one x0 for all chunks).
+    16-bit views are shifted into float32 copies, which take the float32 route at ``precision``.
     Returns (moments, x0 or None)."""
     if x0 is None:
         cand, ratio = column_pilot(views)

@@ -13,8 +13,9 @@
  *     ccab_gesvj which synchronise it once per Jacobi sweep to read the convergence flag;
  *   - return 0 = OK, <0 = bad argument / unsupported, >0 = cudaError_t.  ccab_last_error() gives the
  *     message of the last failure on the calling thread.  No C++ exception crosses the ABI.
- *   - dtype: CCAB_F32 / CCAB_F64.  There is no CPU fallback: without a sm_90a device every compute
- *     entry point fails.
+ *   - dtype: CCAB_F32 / CCAB_F64.  The 16-bit codes CCAB_BF16 / CCAB_F16 are accepted by ccab_moments,
+ *     ccab_moments_workspace_bytes, ccab_column_pilot and ccab_shift_rows only; every other entry point rejects them
+ *     as a bad dtype.  There is no CPU fallback: without a sm_90a device every compute entry point fails.
  */
 #ifndef CCAB200_H
 #define CCAB200_H
@@ -28,12 +29,18 @@ extern "C" {
 
 #define CCAB_F32 0
 #define CCAB_F64 1
+#define CCAB_BF16 2 /* bfloat16 views: the moments and the pilot / shift of the shifted accumulation only */
+#define CCAB_F16 3  /* float16 views: likewise */
 
 /* arithmetic of the moment kernel (ccab_moments `precision`) */
 #define CCAB_PREC_TF32 0   /* fp32 in, one wgmma TF32 pass, fp32 accumulate               */
 #define CCAB_PREC_TF32X3 1 /* fp32 in, hi/lo split + 3 wgmma passes: fp32-grade accuracy          */
 #define CCAB_PREC_EXACT 2  /* FMA in the input dtype on CUDA cores (the only choice for CCAB_F64)  */
 #define CCAB_PREC_TF32X3B 3 /* 3xTF32 with the two cross terms as bf16 MMAs: fp32-grade, 2/3 the tensor work */
+/* For CCAB_BF16 / CCAB_F16 views, CCAB_PREC_TF32, _TF32X3 and _TF32X3B all select the one 16-bit wgmma kernel: the
+ * product of two bf16 or two fp16 values is exact in fp32, so there is nothing to split.  Its fp32 accumulator runs
+ * span at most 2048 samples and are summed in float64, as in the 3xTF32 modes.  CCAB_PREC_EXACT converts on load and
+ * runs FMA in fp32 on CUDA cores, with the same 2048-sample runs folded into float64. */
 
 #define CCAB_MAX_VIEWS 8
 
@@ -53,8 +60,8 @@ int64_t ccab_launch_count(void);
  * np.cov(...) cca_zoo/linear/_mcca.py:150-152,166 and cca_zoo/linear/_gcca.py:101,
  * z.T @ z cca_zoo/deep/objectives.py:86-92; the column sums replace v.mean(axis=0) cca_zoo/_base.py:97.
  * views[v]: device pointer to an n_rows x dims[v] row-major array with leading dimension lds[v]
- * (TF32 paths read the views with TMA: they need 16-byte aligned pointers and lds[v] % 4 == 0, and return -1
- * otherwise). */
+ * (tensor-core paths read the views with TMA: they need 16-byte aligned pointers and a row pitch that is a multiple of
+ * 16 bytes -- lds[v] % 4 == 0 for float32, lds[v] % 8 == 0 for bf16 / fp16 -- and return -1 otherwise). */
 int64_t ccab_moments_size(int n_views, const int64_t* dims);
 int64_t ccab_moments_padded_dim(int n_views, const int64_t* dims);
 size_t ccab_moments_workspace_bytes(int dtype, int precision, int n_views, const int64_t* dims, int64_t n_rows);
@@ -67,9 +74,12 @@ int ccab_moments(int dtype, int precision, int n_views, const void* const* views
  * covariance is eps_prod * (mean / std)^2, eps_prod ~ 1e-7 .. 1e-6 for float32 inputs.  The reference centres the data
  * first (cca_zoo/_base.py:96-99); covariance being shift invariant, the same is had in one pass by accumulating the
  * moments of X - x0 and rebuilding the raw moments in float64:
- *   ccab_column_pilot   x0[j] = mean of column j over the first `rows` rows (device, in the view's dtype);
+ *   ccab_column_pilot   x0[j] = mean of column j over the first `rows` rows (device, in the view's dtype; float32
+ *                       for 16-bit views);
  *                       ratio_max_dev[0] = max(ratio_max_dev[0], max_j mean_j^2 / var_j)   (zero it first)
- *   ccab_shift_rows     Xs = X - x0   (one extra pass, only taken when the pilot says it matters)
+ *   ccab_shift_rows     Xs = X - x0   (one extra pass, only taken when the pilot says it matters; Xs is float32 for
+ *                       16-bit views, whose shifted copy then takes the float32 moment route and whose
+ *                       ccab_moments_unshift runs with dtype CCAB_F32)
  *   ccab_moments        ... on Xs ...
  *   ccab_moments_unshift  M += x0 s^T + s x0^T + n x0 x0^T, s += n x0 in float64 (x0: per view device pointers or NULL)
  * after which the buffer holds the raw moments again: additive over row shards, all-reducible, whatever x0 each rank
