@@ -22,13 +22,17 @@ loss stage runs on the global moments with the global count N read on the device
 ``ccab_covariance_ndev``).  The loss is the loss of the concatenated global batch, replicated on every rank; each rank's
 backward is the exact derivative of that loss with respect to its own rows, centred by the saved global means, with no
 collective (``ccab_ccaloss_bwd_global``, ``ccab_row_sub_scale``).  Every route decision is taken from exchanged data, so
-all ranks take the same route and raise at the same call.
+all ranks take the same route and raise at the same call.  TCCALoss needs a second exchange: after the moments, the
+local contraction of the whitened rows and, for 3 or more views, its marginals are summed with one all-reduce; its
+backward then takes every global row sum from the global tensor and those marginals, again with no collective (see
+``_TCCALossGlobalFn``).
 
-bfloat16 / float16 representations (an encoder under ``torch.autocast``; CCALoss / MCCALoss / GCCALoss) take the
-global-batch route also in a single process, where nothing is exchanged and N is a device scalar holding n: the moment
-pass reads the 16-bit representations as they are (16-bit wgmma, or fp32 FMA for narrow batches), the loss stage runs
-in float32, and the backward runs the float32 global backward on float32 copies of the saved representations made
-inside ``backward``; the gradients come back in the representation's dtype.
+bfloat16 / float16 representations (an encoder under ``torch.autocast``; all four losses) take the global-batch route
+also in a single process, where nothing is exchanged and N is a device scalar holding n: the moment pass reads the
+16-bit representations as they are (16-bit wgmma, or fp32 FMA for narrow batches), the loss stage runs in float32
+and returns a float32 loss, and the backward runs the float32 global backward on float32 copies of the saved
+representations made inside ``backward`` (TCCALoss: every stage after the moment pass in float64, on float64 copies
+made inside ``forward``); the gradients come back in the representation's dtype.
 """
 from __future__ import annotations
 
@@ -740,6 +744,25 @@ def _tcca_eigen_whiten(C, z64, off, dims, eps):
     return H, parts
 
 
+def _tcca_cholesky_factors(C, off, dims, eps):
+    """L_i^-1 with S_i = C_ii + eps I = L_i L_i^T (batched when the widths agree); C stays intact for the eigen route.
+    Returns the factors and their Cholesky status tensors."""
+    m = len(dims)
+    if len(set(dims)) == 1:                        # one batched factorisation for all views
+        S = torch.stack([C[off[i]:off[i + 1], off[i]:off[i + 1]] for i in range(m)])
+        S.diagonal(dim1=1, dim2=2).add_(eps)
+        L, info = ops.potrf_inv_(S, pivot_tol=0.25 * eps)
+        return [L[i] for i in range(m)], [info]
+    Linv, flags = [], []
+    for i in range(m):
+        S = C[off[i]:off[i + 1], off[i]:off[i + 1]].clone()
+        S.diagonal().add_(eps)
+        L, info = ops.potrf_inv_(S, pivot_tol=0.25 * eps)
+        Linv.append(L)
+        flags.append(info)
+    return Linv, flags
+
+
 class _TCCALossFn(torch.autograd.Function):
     """-||M||_F, M = (1/n) sum_s H_1[s] x ... x H_m[s], in float64 for every input dtype (see TCCALoss)."""
 
@@ -759,19 +782,7 @@ class _TCCALossFn(torch.autograd.Function):
         if eigen and not bool(torch.isfinite(C).all()):       # the eigen route reads back anyway
             raise ValueError("TCCALoss: a representation contained NaN or infinity.")
         if not eigen:
-            Linv, flags = [], []
-            if len(set(dims)) == 1:                    # one batched factorisation for all views
-                S = torch.stack([C[off[i]:off[i + 1], off[i]:off[i + 1]] for i in range(m)])
-                S.diagonal(dim1=1, dim2=2).add_(eps)
-                L, info = ops.potrf_inv_(S, pivot_tol=0.25 * eps)
-                Linv, flags = [L[i] for i in range(m)], [info]
-            else:
-                for i in range(m):
-                    S = C[off[i]:off[i + 1], off[i]:off[i + 1]].clone()    # C stays intact for the eigen route
-                    S.diagonal().add_(eps)
-                    L, info = ops.potrf_inv_(S, pivot_tol=0.25 * eps)
-                    Linv.append(L)
-                    flags.append(info)
+            Linv, flags = _tcca_cholesky_factors(C, off, dims, eps)
             flags.append((~torch.isfinite(C).all()).to(torch.int32).reshape(1))
             flags = torch.cat(flags)
             # H_i = Zc_i R_i with R_i = L_i^-T: centring commutes with the right factor
@@ -831,6 +842,151 @@ class _TCCALossFn(torch.autograd.Function):
         return (None, None, None, None, *grads)
 
 
+def _unfolding_products(M, dims, i, pbar=None):
+    """(M_(i) M_(i)^T, M_(i) vec(pbar) or None) for the mode-i unfolding M_(i) (k_i x prod_{j != i} k_j, the other
+    modes in C order, as ``tcca_moment`` orders the marginal pbar).  Both are one two-view contraction over the
+    prod_{j != i} k_j positions on ``tcca_moment``, whose sample splits spread that long reduction over the GPU (a GEMM
+    with a k_i x k_i output would run it in one CTA): X^T [X | vec(pbar)] with X = M_(i)^T, one copy of M."""
+    k, Q = dims[i], M.numel() // dims[i]
+    Y = torch.empty((Q, k if pbar is None else k + 1), dtype=M.dtype, device=M.device)
+    Y[:, :k] = M.reshape(dims).movedim(i, -1).reshape(Q, k)
+    if pbar is not None:
+        Y[:, k] = pbar.reshape(-1)
+    G = ops.tcca_moment([Y[:, :k], Y], scale=1.0)
+    return G[:, :k], (G[:, k] if pbar is not None else None)
+
+
+def _tcca_sizes(dims):
+    """Entries of M and of the marginals P_i = sum_s (x)_{j != i} H_j[s] (sent for m >= 3 only: for m = 2, P_i is the
+    column sum of a view centred with the global mean, which is 0)."""
+    P = 1
+    for d in dims:
+        P *= d
+    return P, ([P // d for d in dims] if len(dims) >= 3 else [])
+
+
+class _TCCALossGlobalFn(torch.autograd.Function):
+    """TCCALoss of the global batch: this rank's rows, the moments and the cross-moment tensor of all ranks (see the
+    module docstring).  With ``exchange=False`` (16-bit representations in a single process) the same body without the
+    exchanges, N a device scalar holding n.
+
+    Forward: exchange 1 (moments) gives the global C and means mu_i; the whitening (Cholesky R_i = L_i^-T, or the
+    eigen route W_i) and H_i = (z_i - mu_i) R_i are replicated / local; exchange 2 sums [sum_s (x)_i H_i[s] | P_i] over
+    the ranks, scaled by 1/N on the device to [M | Pbar_i].  Backward, with Gamma_i = coef Y_i, coef = -g / (N ||M||)
+    and Y_i the adjoint of the global M against the local H_j, every global row sum follows from M and Pbar_i:
+        T_i = sum H_i^T Gamma_i = coef N M_(i) M_(i)^T,   (1/N) sum Gamma_i = r_i = coef M_(i) vec(Pbar_i),
+        Cholesky: dL/dz_i = (Gamma_i - H_i T_i / (N - 1) - 1 r_i^T) R_i^T,
+        eigen:    dL/dz_i = Gamma_i W_i + 2/(N - 1) Zc_i X_i - 1 r_i^T W_i,  X_i from B_i = W_i^-1 T_i,
+    so the backward issues no collective."""
+
+    @staticmethod
+    def forward(ctx, eps, precision, status, sync, group, exchange, *zs):
+        in_dt = zs[0].dtype
+        n, m = int(zs[0].shape[0]), len(zs)
+        zd = [_row_major(z) for z in zs]
+        dims = [int(z.shape[1]) for z in zd]
+        off = [0]
+        for d in dims:
+            off.append(off[-1] + d)
+        dev = zd[0].device
+        mom, n_dev = _exchange(zd, _resolve_precision(precision, zd), group, exchange)
+        C, mean = ops.covariance(mom, dims, n_dev, center=True, dtype=torch.float64)
+        width = max(dims)
+        # n - 1 >= width here implies N - 1 >= width: no read-back.  Only a narrower shard reads N, and N (exchanged)
+        # decides for every rank alike.
+        eigen = n - 1 < width and _global_count(n_dev, "TCCALoss") - 1 < width
+        if not eigen:
+            Linv, flags = _tcca_cholesky_factors(C, off, dims, eps)
+            flags = torch.cat(flags + [(~torch.isfinite(C).all()).to(torch.int32).reshape(1)])
+            if sync:
+                f = flags.tolist()                     # flags of the global C: the same on every rank
+                if f[-1]:
+                    raise ValueError("TCCALoss: a representation contained NaN or infinity.")
+                eigen = any(f[:-1])
+            else:
+                status.push(flags)
+        z64 = [z.to(torch.float64, copy=True) for z in zd]
+        one = torch.ones(1, dtype=torch.float64, device=dev)
+        if eigen:
+            _global_count(n_dev, "TCCALoss")
+            _check_finite(C, "TCCALoss")
+            if not exchange and in_dt != torch.float64:
+                # the clamp at eps is decided on the eigenvalues: float64 moments of the float64 copies, as the
+                # per-replica route takes them (with an exchange, the exchanged moments are all there is)
+                C, mean = ops.covariance(ops.moments(z64), dims, n, center=True, dtype=torch.float64)
+        H, saved = [], []
+        for i, d in enumerate(dims):
+            Zc = z64[i]
+            if n:
+                ops.row_sub_scale_(Zc, mean[off[i]:off[i + 1]], one)       # centred with the global mean
+            if eigen:
+                lam, Vt = ops.syevj(C[off[i]:off[i + 1], off[i]:off[i + 1]].clone())
+                Wt, g, _ = ops.whiten_rows(lam, Vt, 0.0, floor_add=eps, rank_tol=-1.0, lam_floor=0.0)
+                W = ops.gemm(Vt, Wt, transa=True)
+                Winv = ops.gemm(Vt, ops.scale(Vt, rows=g, rows_pow=-1), transa=True)    # V clamp(Lam, eps)^1/2 V^T
+                H.append(ops.gemm(Zc, W) if n else Zc)
+                saved += [Zc, W, Vt, _tcca_divided_differences(lam + eps, eps), Winv]
+            else:
+                H.append(ops.gemm(Zc, Linv[i], transb=True) if n else Zc)        # R_i = L_i^-T
+                saved.append(Linv[i])
+        P, marg = _tcca_sizes(dims)
+        buf = (torch.empty if n else torch.zeros)(P + sum(marg), dtype=torch.float64, device=dev)
+        if n:                                          # no rows here: zeros, and no kernel on an empty batch
+            ops.tcca_moment(H, scale=1.0, out=buf[:P])
+            o = P
+            for i, q in enumerate(marg):
+                ops.tcca_moment([H[j] for j in range(m) if j != i], scale=1.0, out=buf[o:o + q])
+                o += q
+        if exchange:
+            parallel.allreduce_sum_(buf, group)
+        row = buf.view(1, -1)
+        ops.scale(row, rows=n_dev, rows_pow=-1, out=row)                  # [M | Pbar_i]: sums over all ranks / N
+        norm = ops.frobenius_norm(buf[:P].view(dims[0], -1))
+        ctx.m, ctx.dims, ctx.in_dt, ctx.eigen = m, dims, in_dt, eigen
+        ctx.save_for_backward(buf, norm, n_dev, *H, *saved)
+        return (-norm).reshape(()).to(_compute_dtype(in_dt)).clone()
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        m, dims, in_dt = ctx.m, ctx.dims, ctx.in_dt
+        buf, norm, n_dev, *t = ctx.saved_tensors
+        H, rest = t[:m], t[m:]
+        head = (None,) * 6
+        if H[0].shape[0] == 0:
+            return (*head, *[torch.zeros((0, d), dtype=in_dt, device=buf.device) for d in dims])
+        P, marg = _tcca_sizes(dims)
+        M = buf[:P]
+        go = grad_out.to(torch.float64).reshape(1)
+        cN = torch.where(norm > 0, -go / norm, torch.zeros_like(norm))   # coef N; 0 at ||M|| = 0
+        coef = cN / n_dev
+        one = torch.ones(1, dtype=torch.float64, device=buf.device)
+        gam = ops.tcca_moment_adjoint(M, list(H), scale_dev=coef)
+        grads, o = [], P
+        for i in range(m):
+            G, r = _unfolding_products(M, dims, i, buf[o:o + marg[i]] if marg else None)
+            if r is not None:                                               # r_i = coef M_(i) vec(Pbar_i)
+                r = r * coef
+                o += marg[i]
+            g = gam[i]
+            if ctx.eigen:
+                Zc, W, Vt, F, Winv = rest[5 * i:5 * i + 5]
+                B = ops.gemm(Winv, G) * cN                                  # sum over all rows of Zc_i^T Gamma_i
+                B = 0.5 * (B + B.T)
+                X = ops.gemm(Vt, F * ops.gemm(ops.gemm(Vt, B), Vt, transb=True), transa=True)
+                X = ops.gemm(X, Vt) * (2.0 / (n_dev - 1.0))
+                out = ops.gemm(g, W)
+                ops.gemm(Zc, X, beta=1.0, out=out)
+                if r is not None:
+                    ops.row_sub_scale_(out, ops.gemm(r.reshape(1, -1), W).reshape(-1), one)
+            else:
+                ops.gemm(H[i], G * (cN / (n_dev - 1.0)), alpha=-1.0, beta=1.0, out=g)
+                if r is not None:
+                    ops.row_sub_scale_(g, r, one)
+                out = ops.gemm(g, rest[i])                                  # R_i^T = L_i^-1
+            grads.append(out.to(in_dt))
+        return (*head, *grads)
+
+
 class TCCALoss(nn.Module):
     r"""Deep tensor-CCA loss for 2 to 8 views (cca_zoo/deep/objectives.py:223-289): :math:`-\|M\|_F` with
     :math:`M = \frac1n \sum_s H_1[s] \otimes \cdots \otimes H_m[s]` the cross-moment tensor of the whitened
@@ -855,15 +1011,33 @@ class TCCALoss(nn.Module):
         verify: ``"lazy"`` (default) reads nothing back: the Cholesky status and a NaN flag are inspected at the next
             call or by ``check()``.  ``"sync"`` reads them back in every call, raises ``ValueError`` on NaN or
             infinity and takes the eigen route for a batch whose S_i is not numerically positive definite.
+        global_batch: under data parallelism (an initialised process group of more than one rank), compute the loss
+            of the concatenated global batch instead of each replica's own: the block moments are summed over the
+            ranks, then the local contraction of the whitened rows (and, for 3 or more views, its marginals), so a
+            forward runs two exchanges; every rank gets the same loss, and each rank's backward (no collective) is
+            the exact derivative of that loss with respect to its own rows.  A rank may hold 0 rows.  DDP averages
+            parameter gradients over the W ranks, so they come out as (1/W) dL_global/dθ.  Without a process group,
+            or with one rank, the per-replica route runs unchanged.  Default False (the reference's per-replica
+            statistics).
+        process_group: the ranks whose batches form the global batch (``None``: the default group, as in
+            ``torch.nn.SyncBatchNorm``).
+
+    Representations may be float32, float64, bfloat16 or float16 (all of one dtype).  16-bit representations are read
+    by the moment pass as they are and take the global-batch route (without an exchange in a single process);
+    everything after the moment pass runs in float64, the loss is float32 and the gradients have the representations'
+    dtype.
     """
 
-    def __init__(self, eps: float = 1e-5, precision: str = "auto", verify: str = "lazy") -> None:
+    def __init__(self, eps: float = 1e-5, precision: str = "auto", verify: str = "lazy", global_batch: bool = False,
+                 process_group=None) -> None:
         super().__init__()
         if verify not in ("lazy", "sync"):
             raise ValueError("verify must be 'lazy' or 'sync'")
         self.eps = eps
         self.precision = precision
         self.verify = verify
+        self.global_batch = global_batch
+        self.process_group = process_group
         self._status = _LazyStatus("TCCALoss")
 
     def check(self) -> None:
@@ -876,12 +1050,14 @@ class TCCALoss(nn.Module):
             raise ValueError(f"TCCALoss takes 2 to {ops.TCCA_MAX_VIEWS} representations, got {len(zs)}.")
         _require_cuda("TCCALoss", *zs)
         dt = zs[0].dtype
-        if dt not in (torch.float32, torch.float64) or any(z.dtype != dt for z in zs):
-            raise ValueError("representations must share a float32/float64 dtype")
+        if dt not in _LOSS_DTYPES or any(z.dtype != dt for z in zs):
+            raise ValueError("representations must share a float32/float64/bfloat16/float16 dtype")
         if any(z.dim() != 2 for z in zs) or any(z.shape[0] != zs[0].shape[0] for z in zs):
             raise ValueError("representations must be 2-D with the same number of rows")
+        # every argument error is raised here, before any exchange; a global batch checks N >= 2 from exchanged data
+        glob = _is_global(self.global_batch, self.process_group)
         n = int(zs[0].shape[0])
-        if n < 2:
+        if n < 2 and not glob:
             raise ValueError(f"TCCALoss needs at least 2 samples for a covariance, got n = {n}.")
         entries = 1
         for z in zs:
@@ -892,4 +1068,7 @@ class TCCALoss(nn.Module):
             raise ValueError(f"the cross-moment tensor of widths {[int(z.shape[1]) for z in zs]} has {entries} entries; "
                              f"TCCALoss supports at most 2^25 = {ops.TCCA_MAX_ENTRIES} (the product of the widths).")
         self._status.poll()
+        if glob or dt in HALF_DTYPES:
+            return _TCCALossGlobalFn.apply(float(self.eps), self.precision, self._status, self.verify == "sync",
+                                           self.process_group, glob, *zs)
         return _TCCALossFn.apply(float(self.eps), self.precision, self._status, self.verify == "sync", *zs)

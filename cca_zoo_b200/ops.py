@@ -926,10 +926,12 @@ TCCA_MAX_ITER = 100            # tensorly's n_iter_max
 TCCA_HEADER = 8                # doubles in front of the rec history in the state block of ccab_tcca_fit
 
 
-def tcca_moment(Z, nsplit: int = 0):
+def tcca_moment(Z, nsplit: int = 0, scale: float | None = None, out=None):
     """M = Z_1^T KR(Z_2, ..., Z_m) / n (p_1 x prod_{i>1} p_i float64, CUDA): the mode-0 unfolding of the cross-moment
     tensor of the float64 (n, p_i) CUDA tensors ``Z`` (ccab_tcca_moment).  ``nsplit`` > 0 forces that many sample
-    splits; 0 lets the library choose from the shape."""
+    splits; 0 lets the library choose from the shape.  ``scale`` replaces the factor 1/n (1.0: the unscaled sum over
+    the samples); ``out``, a contiguous float64 CUDA tensor of p_1 * prod_{i>1} p_i entries, receives M in place of a
+    new tensor."""
     lib = _lib.load()
     for i, z in enumerate(Z):
         _require_cuda(z, f"Z[{i}]")
@@ -944,11 +946,18 @@ def tcca_moment(Z, nsplit: int = 0):
     P = 1
     for p in dims[1:]:
         P *= p
-    M = torch.empty((dims[0], P), dtype=torch.float64, device=Z[0].device)
+    if out is None:
+        M = torch.empty((dims[0], P), dtype=torch.float64, device=Z[0].device)
+    else:
+        _require_cuda(out, "out")
+        if out.dtype != torch.float64 or out.numel() != dims[0] * P or not out.is_contiguous():
+            raise ValueError(f"tcca_moment: `out` must be a contiguous float64 tensor of {dims[0] * P} entries")
+        M = out
     ws = _ws(lib.ccab_tcca_moment_workspace_bytes(len(dims), d, n, int(nsplit)), M.device)
     ptrs = (C.c_void_p * len(Z))(*[z.data_ptr() for z in Z])
+    f = 1.0 / max(n, 1) if scale is None else float(scale)
     with torch.cuda.device(M.device):
-        rc = lib.ccab_tcca_moment(len(dims), d, n, ptrs, _lib.i64_array([z.stride(0) for z in Z]), 1.0 / max(n, 1),
+        rc = lib.ccab_tcca_moment(len(dims), d, n, ptrs, _lib.i64_array([z.stride(0) for z in Z]), f,
                                   int(nsplit), _ptr(M), _ptr(ws), ws.numel(), _stream(M))
     _lib.check(rc, "ccab_tcca_moment")
     return M

@@ -112,6 +112,13 @@ def allreduce_moments_lazy(moments: torch.Tensor, n_local: int, group=None, dims
     return packed[:-1], None, packed[-1:]
 
 
+def allreduce_sum_(buf: torch.Tensor, group=None) -> torch.Tensor:
+    """In place: ``buf`` summed over the ranks of ``group`` with one all-reduce (the tensor exchange of the global-batch
+    ``TCCALoss``); returns ``buf``."""
+    dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=group)
+    return buf
+
+
 def shard_rows(n_rows: int, rank: int, world: int):
     """Contiguous row block [lo, hi) of rank ``rank``."""
     base, rem = divmod(n_rows, world)
